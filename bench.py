@@ -55,6 +55,8 @@ def parse_args():
     ap.add_argument("--workload", default="scan", choices=["scan", "dimer"],
                     help="scan: the headline metric (default); dimer: BASELINE.json configs[4], all-pairs dimer grid")
     ap.add_argument("--primers", type=int, default=100_000, help="primers of the dimer workload")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step computed to DIR/<name>.npy (scan workload, rank 0)")
     return ap.parse_args()
 
 
@@ -68,7 +70,7 @@ def host_cores() -> int:
 
 # ----------------------------------------------------------------------------------------------------------
 class ClockSampler(threading.Thread):
-    """SM clock and throttle reasons during the timed region (B200_PROFILING.md), read through NVML in-process: spawning
+    """SM clock and throttle reasons during the timed region, read through NVML in-process: spawning
     nvidia-smi five times a second initialises every GPU of the box each time and perturbs the ranks it shares them
     with; nvidia-smi is only the fallback when the NVML binding is missing"""
 
@@ -125,17 +127,14 @@ class ClockSampler(threading.Thread):
         sm = sorted(r[0] for r in self.rows)
         names = ["hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"]
         reasons = [n for i, n in enumerate(names) if any(r[2][i] for r in self.rows)]
-        return {"sm_mhz": sm[len(sm) // 2], "sm_max_mhz": self.rows[0][1], "reasons": reasons,
-                "samples": len(self.rows), "source": "nvml" if self.nvml is not None else "nvidia-smi"}
-
-
-def kernel_traffic():
-    """DRAM bytes (read + write) per launch of the profiled kernels, from the committed `ncu --set full` captures"""
-    path = os.path.join(ROOT, "profiles", "r02_traffic.json")
-    if os.path.exists(path):
-        with open(path) as fh:
-            return json.load(fh)
-    return {}
+        out = {"sm_mhz": sm[len(sm) // 2], "sm_max_mhz": self.rows[0][1], "reasons": reasons,
+               "samples": len(self.rows), "source": "nvml" if self.nvml is not None else "nvidia-smi"}
+        if self.nvml is not None:           # a card set below its rated power runs slower: part of the number
+            try:
+                out["power_limit_w"] = self.nvml.nvmlDeviceGetEnforcedPowerLimit(self.handle) / 1000
+            except Exception:
+                pass
+        return out
 
 
 def peaks():
@@ -143,7 +142,52 @@ def peaks():
     if os.path.exists(path):
         with open(path) as fh:
             return float(json.load(fh)["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3)"
+
+
+DUMP_BYTES = 48 << 20           # budget of the bit-vector sample of --dump-outputs (the whole dump stays under 64 MB)
+
+
+def dump_outputs(out_dir, recs, app):
+    """What one design() call returned, as float arrays (the synthetic input is seeded, so two builds can be compared
+    file by file):
+      rows.npy           float64 [rows, 11]: the .out TSV sorted by position — Position, both entropies,
+                         primer_degenerate_number, nonsense_primer_number, Optimal / Mis-F / Mis-R coverage, Tm, then the
+                         Information column as the primer's GC content (computed from the primer where the column holds
+                         notes instead) and a note mask (1 GC_out_of_range, 2 di_nucleotide, 4 hairpin); all finite
+      primers.npy        float32 [rows, k]: Optimal_primer as 4-bit base sets (A=1 C=2 G=4 T=8)
+      bits_positions.npy float64 [n]: window of every primer whose bit vectors were kept (rows before the self-dimer drop)
+      bits_popcount.npy  float64 [n, 3]: set bits of its F non-cover, R non-cover and gap-row vectors over all sequences
+      bits_sample.npy    float32 [n, 3, m]: those bits for a fixed seeded sample of m sequences (bits_sample_seqs.npy)"""
+    import numpy as np
+    from multiprime_b200.core import gc_content
+    from multiprime_b200.iupac import CHAR_CODE
+    os.makedirs(out_dir, exist_ok=True)
+    rows = sorted((r["row"] for r in recs), key=lambda row: row[0])
+    notes = ("GC_out_of_range", "di_nucleotide", "hairpin")
+    table = np.zeros((len(rows), 11), np.float64)
+    primers = np.zeros((len(rows), K), np.float32)
+    for i, row in enumerate(rows):
+        info = row[10]
+        noted = isinstance(info, str)
+        mask = sum(1 << j for j, name in enumerate(notes) if name in info) if noted else 0
+        sets = [CHAR_CODE[c] for c in row[3]]
+        table[i] = row[:3] + row[4:10] + [gc_content(sets) if noted else info, mask]
+        primers[i] = sets
+    pos, bits = app.coverage_bits()
+    n_seq = app.n_local
+    popcount = np.zeros((len(pos), 3), np.float64)
+    for i in range(len(pos)):
+        popcount[i] = np.unpackbits(bits[i].view(np.uint8), axis=1, bitorder="little")[:, :n_seq].sum(axis=1)
+    m = max(1, min(n_seq, 8192, DUMP_BYTES // max(1, 12 * len(pos))))
+    seqs = np.sort(np.random.default_rng(0).choice(n_seq, m, replace=False))
+    sample = ((bits[:, :, seqs >> 5] >> (seqs & 31).astype(np.uint32)) & 1).astype(np.float32)
+    out = {"rows": table, "primers": primers, "bits_positions": pos.astype(np.float64), "bits_popcount": popcount,
+           "bits_sample": sample, "bits_sample_seqs": seqs.astype(np.float64)}
+    for name, arr in out.items():
+        if not np.isfinite(arr).all():
+            raise ValueError("--dump-outputs: %s holds a value that is not finite" % name)
+        np.save(os.path.join(out_dir, name + ".npy"), arr)
 
 
 # ----------------------------------------------------------------------------------------------------------
@@ -372,12 +416,13 @@ def run_b200(args):
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
         t0 = time.perf_counter()
-        nrows = 0
+        recs = []
         per_step = []
         for _ in range(args.steps):
             ts = time.perf_counter()
-            nrows = len(fn())
+            recs = fn()
             per_step.append(1000 * (time.perf_counter() - ts))
+        nrows = len(recs)
         e1.record()
         barrier()
         wall = time.perf_counter() - t0
@@ -397,6 +442,8 @@ def run_b200(args):
             results["candidates"] = app.stats["candidates"] / args.steps
             results["phases"] = {k: round(v / args.steps, 2) for k, v in app.stats["phase_ms"].items()}
             app.ctx.profile(False)
+            if args.dump_outputs and rank == 0:
+                dump_outputs(args.dump_outputs, recs, app)
     evals_all = float(results["evals_per_step"])      # already global: calls x (sequences of ALL shards)
     if world > 1:
         sys.stderr.write("rank %d phases ms/step: %s\n" % (rank, json.dumps(results["phases"])))
@@ -409,14 +456,13 @@ def run_b200(args):
     e2e_ms = results["e2e"]["ms"] / args.steps
     peak, peak_src = peaks()
     prof = results["prof"]
-    traffic = kernel_traffic()
 
     def roofline_of(kn):
         ms, n, units = prof[kn]
         per_unit = BYTES_PER_EVAL if kn == "k_cscan" else BYTES_PER_KMER
         ach = units * per_unit / (ms / 1000) / 1e9 if ms > 0 else 0.0
         return {"bound": "hbm", "kernel": kn, "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak,
-                "traffic": traffic.get(kn), "peak_source": peak_src, "launches": n,
+                "peak_source": peak_src, "launches": n,
                 "avg_launch_ms": ms / max(1, n), "units_in_launches": units, "bytes_per_unit": per_unit,
                 "ms_per_step": ms / args.steps}
 
@@ -425,10 +471,10 @@ def run_b200(args):
     roof["note"] = (
         "dominant kernel of the step by CUDA-event time. achieved = algorithmic bytes (SURVEY.md 8d: k/2 B per (window, "
         "sequence) k-mer for the window passes, k/2 + 0.25 B per candidate x sequence evaluation for the scan) / "
-        "event-timed kernel time; traffic = dram read+write bytes of one launch (ncu --set full, profiles/). The "
+        "event-timed kernel time. The "
         "algorithmic figure assumes no reuse: the window passes cut up to 32 windows out of every loaded word and the "
         "column scan re-reads plane rows from L2, so real DRAM traffic is far below it and a fraction above 1 is "
-        "reuse, not a faster-than-HBM kernel; these kernels are bound by L2 atomics / integer issue (see profiles/README.md)")
+        "reuse, not a faster-than-HBM kernel")
     line = {
         "metric": "candidate_x_sequence_evals_per_sec", "value": value, "unit": "evals/s", "n_gpus": world,
         "steps": args.steps, "warmup": args.warmup, "ms_per_step": ms_step, "higher_is_better": True,
@@ -438,10 +484,11 @@ def run_b200(args):
                                                                   results["value"]["rows"]),
                    "parallelism": "sequence shards x%d: windows owned round-robin (all-to-all of haplotype entries), "
                                   "all-reduce of the coverage-count vector per scan round" % world,
-                   "l2": "inputs (2 x %.0f MB of bit-planes + GB-sized haplotype tables) exceed the 126 MB L2" %
+                   "l2": "inputs (2 x %.0f MB of bit-planes + GB-sized haplotype tables) exceed the 50 MB L2" %
                          (n_seq * n_col / 2 / 1e6),
                    "evals_per_step": evals_all, "scan_rounds_per_step": results["scan_calls"],
                    "scan_candidates_per_step": results["candidates"]},
+        "device": torch.cuda.get_device_name(local),
         "clocks": sampler.summary(),
         "e2e": {"value": evals_all / (e2e_ms / 1000), "unit": "evals/s", "h2d_bytes_per_step": h2d,
                 "d2h_bytes_per_step": int(results["value"]["rows"] * 120), "ms_per_step": e2e_ms,

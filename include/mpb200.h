@@ -1,5 +1,5 @@
 /*
- * mpb200.h — C ABI of libmpb200.so, the B200 (sm_100a) implementation of multiPrime's degenerate-primer
+ * mpb200.h — C ABI of libmpb200.so, the H100 (sm_90a) implementation of multiPrime's degenerate-primer
  * candidate scan.  Loaded from Python with ctypes (multiprime_b200/_lib.py); no torch / C++ types cross
  * this boundary: plain pointers, sizes and opaque handles only.
  *

@@ -1,4 +1,4 @@
-"""ctypes binding of libmpb200.so (include/mpb200.h).  No CPU fallback: every compute call needs a B200."""
+"""ctypes binding of libmpb200.so (include/mpb200.h).  No CPU fallback: every compute call needs an H100."""
 from __future__ import annotations
 
 import ctypes as C

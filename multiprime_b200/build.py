@@ -1,4 +1,5 @@
-"""Build libmpb200.so in-tree with nvcc for sm_100a (no JIT cache: the .so must travel with the repo snapshot)."""
+"""Build libmpb200.so in-tree with nvcc for sm_90a (H100).  The library lives next to this file, so the package is
+importable and runnable straight from the source tree once this has run."""
 from __future__ import annotations
 
 import os
@@ -33,7 +34,7 @@ def needs_build() -> bool:
 def build(force: bool = False, verbose: bool = False) -> str:
     if not force and not needs_build():
         return LIB
-    cmd = [nvcc_path(), "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    cmd = [nvcc_path(), "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
            "-Xptxas", "-v" if verbose else "-O3", "-shared", "-Xcompiler", "-fPIC", "-cudart", "static", "-t", "5",
            "-I", os.path.join(ROOT, "include"), "-I", CSRC, "-o", LIB] + [os.path.join(CSRC, s) for s in SOURCES]
     res = subprocess.run(cmd, capture_output=True, text=True)

@@ -2,7 +2,7 @@
 
 `NN_degenerate` keeps the reference's constructor arguments, `run()` and output files (core:343-365,
 1133-1180).  All per-sequence work — window extraction with gap patching, haplotype counting, base / dinucleotide
-tensors, the mismatch scan, Tm — runs in libmpb200.so on a B200; this module holds the per-window control logic
+tensors, the mismatch scan, Tm — runs in libmpb200.so on an H100; this module holds the per-window control logic
 (gates, seeds, the NN-array refinement walk, filters, writers), which only ever touches O(k) numbers per window.
 
 There is no CPU fallback: constructing NN_degenerate without a CUDA device raises.
@@ -979,9 +979,9 @@ def exact_mean(vals) -> float:
 
 
 def _default_batch(n_seq: int) -> int:
-    # table bytes per window = 20 * 2^ceil(log2(2n+64)); keep a batch under ~48 GB of the 180 GB HBM
+    # table bytes per window = 20 * 2^ceil(log2(2n+64)); keep a batch under ~32 GB of the 80 GB HBM
     cap = 1 << max(6, int(math.ceil(math.log2(2 * n_seq + 64))))
-    return max(1, min(4096, int(48e9 // (20 * cap))))
+    return max(1, min(4096, int(32e9 // (20 * cap))))
 
 
 def _near_half(x: float) -> bool:

@@ -1,5 +1,5 @@
-// mpb200.cu — libmpb200.so: kernels + C ABI (include/mpb200.h) of the B200 degenerate-primer candidate scan.
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -lineinfo -O3 -shared -Xcompiler -fPIC (see build.py)
+// mpb200.cu — libmpb200.so: kernels + C ABI (include/mpb200.h) of the H100 degenerate-primer candidate scan.
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo -O3 -shared -Xcompiler -fPIC (see build.py)
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdarg.h>
@@ -67,8 +67,9 @@ extern "C" int mpb_ctx_create(int device, mpb_ctx** out) {
     CK(cudaSetDevice(device));
     cudaDeviceProp prop;
     CK(cudaGetDeviceProperties(&prop, device));
-    if (prop.major < 10) return fail(MPB_ECUDA, "device %d is sm_%d%d; libmpb200 is built for sm_100a only", device,
-                                     prop.major, prop.minor);
+    if (prop.major != 9 || prop.minor != 0)
+        return fail(MPB_ECUDA, "device %d is sm_%d%d; libmpb200 is built for sm_90a (H100) only", device, prop.major,
+                    prop.minor);
     cudaMemPool_t pool;
     CK(cudaDeviceGetDefaultMemPool(&pool, device));
     uint64_t thr = UINT64_MAX;
@@ -507,7 +508,7 @@ extern "C" int mpb_seq_attr(mpb_msa* m, int32_t* lead_hd, int32_t* rstrip_hd) {
 //   * Windows are grouped by column word (mpb_window_groups: consecutive batch entries with the same p >> 5, at most
 //     32): all of them cut their k-mers out of the same two 128-bit plane words of a sequence, so a thread loads the
 //     two words once per tile and funnel-shifts up to 32 windows out of them (round 1 and the first version of this
-//     round re-read them per window: 18.6 GB of L2 traffic per pass, and 73 % of the stall samples waiting for it).
+//     round re-read them per window, many GB of L2 traffic per pass).
 //   * Block (x, y) owns WIN_TILES x 256 sequences and walks the groups y, y + gridDim.y, ...; a warp owns 32
 //     sequences per tile, and LANE j of the warp keeps the running state of WINDOW j of the group.  In a window below
 //     the entropy gate most sequences carry the SAME k-mer, so the warp keeps that majority k-mer and its count in
@@ -783,7 +784,7 @@ k_hist(const uint32_t* __restrict__ pl, int64_t nsp, int64_t n_seq, const int32_
     __shared__ int s_p[HIST_THREADS / 32][32];                      // window start columns of the group, per warp
     __shared__ unsigned long long s_major[HIST_THREADS / 32][32];   // majority key of every window of the group, per warp
     // minority rows wait in a per-warp queue and are inserted 32 at a time: a table insert is three dependent trips to
-    // L2, and done where the row stands it ran with ~5 of 32 lanes (ncu: 35 % of the stall samples at the first of them)
+    // L2, and done where the row stands it runs with a few of the 32 lanes
     __shared__ unsigned long long s_qkey[HIST_THREADS / 32][HIST_QCAP];
     __shared__ unsigned int s_qmeta[HIST_THREADS / 32][HIST_QCAP];  // window index | row within the block << 16
     unsigned qn = 0;
@@ -950,7 +951,7 @@ k_prefilter_sums(const unsigned int* __restrict__ bins, double* __restrict__ s0,
 // column-domain window passes
 // ------------------------------------------------------------------------------------------------------
 // The row-domain passes above spend ~80 (prefilter) / ~210 (tables) warp instructions per (window, 32 rows) to find out,
-// row by row, that most rows of a conserved window carry the same k-mer (ncu: both issue-bound at ~44 %).  On the column
+// row by row, that most rows of a conserved window carry the same k-mer (both are instruction-issue bound).  On the column
 // view (colp: one bit per sequence, 32 sequences per word) that question is an AND: with lane = column and a word of 32
 // rows per warp, "row equals the reference k-mer R_w of window w" is the AND over the window's columns of
 // plane[column][base R_w has there] — a sliding AND over k lanes, done for all windows that start in the lanes' columns
@@ -2008,7 +2009,7 @@ extern "C" int mpb_hist_exceptions(mpb_hist* h, int64_t max_n, int32_t* win_idx,
 // One chunk (CNT candidates of one window, masks in registers) against the block's sequence tiles.
 // Rows that need more than the funnel shift — the window starts / ends inside a gap run, holds IUPAC cells, or runs
 // past a ragged row — are "special" (about 0.5 % of the rows).  Handling them inline left most of the warp idle for
-// hundreds of instructions (profiles/README.md, stage r01-a/e), so when DEFER is set they are only recorded in a
+// hundreds of instructions, so when DEFER is set they are only recorded in a
 // block-private list and evaluated densely, one per thread, after the block has walked all its chunks.
 template <bool BITS, int CNT>
 __device__ __forceinline__ void scan_chunk(const uint32_t* __restrict__ pl, int64_t nsp, int64_t n_seq,

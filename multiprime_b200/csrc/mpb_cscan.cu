@@ -129,8 +129,7 @@ k_cscan(const uint32_t* __restrict__ colp, long long nwords, int v, const uint32
         const uint32_t* psf = sp + sp[7];
         const uint32_t* psr = psf + nsf;
         unsigned n0 = 0, nf = 0, nr = 0, nt = 0;
-        // two words per pass: their plane loads are independent, so twice as many are in flight per thread (the first
-        // version, one word at a time, spent 60 % of its stall samples waiting for them)
+        // two words per pass: their plane loads are independent, so twice as many are in flight per thread
 #pragma unroll 1
         for (int j = 0; j < CSCAN_WPT; j += 2) {
             const long long wa = w0 + (long long)j * CSCAN_THREADS;

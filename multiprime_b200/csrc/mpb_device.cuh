@@ -3,7 +3,7 @@
 //     core:666-687, restated for bit-planes),
 //   * IUPAC expansion in the reference's product order (core:105-107, 368-380),
 //   * 64-bit haplotype keys and the open-addressing table insert.
-// sm_100a only.
+// sm_90a only.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

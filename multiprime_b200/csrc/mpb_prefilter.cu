@@ -6,7 +6,7 @@
 // below, and a window whose bound is above the gate never needs a haplotype table.
 //
 // How: the row-domain kernel (k_prefilter in mpb200.cu) pays ~80 warp instructions per (window, 32 rows) and one global
-// reduction per minority row — 3.8e8 L2 reductions per pass on the 10^6 x 600 workload, which bound it (3.5 ms).  Here
+// reduction per minority row — hundreds of millions of L2 reductions per pass on the 10^6 x 600 workload.  Here
 //   * one CLUSTER of BS_CLUSTER thread blocks owns one window; each block keeps the window's whole histogram in shared
 //     memory (8192 bins) for its share of the rows — no global atomics at all;
 //   * a thread takes 32 sequences at a time (one word of the column view) and walks the window's k columns once: the row

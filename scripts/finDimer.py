@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""drop-in for the reference's scripts/finDimer.py: same flags and output files, computed by libmpb200 on a B200
+"""drop-in for the reference's scripts/finDimer.py: same flags and output files, computed by libmpb200 on an H100
 (point the Snakemake `scripts_dir` at this directory)"""
 import os
 import sys

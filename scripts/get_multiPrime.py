@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """drop-in for the reference's scripts/get_multiPrime.py: same flags and output files, dimer check and pair coverage
-by libmpb200 on a B200 (point the Snakemake `scripts_dir` at this directory)"""
+by libmpb200 on an H100 (point the Snakemake `scripts_dir` at this directory)"""
 import os
 import sys
 
