@@ -307,6 +307,9 @@ extern "C" int mpb_msa_upload(mpb_ctx* ctx, const uint8_t* packed4, int64_t n_se
         return fail(MPB_EINVAL, "bad shape n_seq=%lld n_col=%lld row_bytes=%lld", (long long)n_seq, (long long)n_col,
                     (long long)row_bytes);
     if (n_seq >= (1ll << 31)) return fail(MPB_EINVAL, "n_seq must be < 2^31");
+    // k_build_colp puts one 32-column word per blockIdx.y
+    if ((n_col + 31) / 32 > 65535)
+        return fail(MPB_EINVAL, "n_col=%lld: at most 65535 x 32 = 2097120 columns are supported", (long long)n_col);
     CK(cudaSetDevice(ctx->device));
     mpb_msa* m = new mpb_msa;
     memset(m, 0, sizeof *m);

@@ -399,37 +399,47 @@ extern "C" int mpb_cscan(mpb_hist* h, uint32_t fmask, uint32_t rmask, const mpb_
 // does an expansion of this primer occur in this sequence".  On the column view that is the scan kernel with the window
 // start as a free variable: thread = (position, 32-sequence word); the running AND of the per-column match words dies
 // after two or three columns almost everywhere.  Hits are rare and leave as (pattern, sequence, position) triples.
+// A cell matches only when it holds exactly one base and that base is allowed: an IUPAC cell sets two or more planes
+// and the reference's plain-text search never matches it.  Columns are walked with stride gridDim.y (capped at 65535),
+// so lines of any width fit one launch.
 struct mpb_pattern {
     uint32_t allow[4];
     int32_t len;
 };
+
+#define PATTERN_MAX_GY 65535
 
 __global__ void __launch_bounds__(256)
 k_pattern_hits(const uint32_t* __restrict__ colp, long long nwords, int n_col, const mpb_pattern* __restrict__ pats, int n_pat,
                long long max_hits, int32_t* __restrict__ hit_pat, int32_t* __restrict__ hit_row, int32_t* __restrict__ hit_pos,
                unsigned long long* __restrict__ n_hits) {
     const long long w = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    const int x = blockIdx.y;
     if (w >= nwords) return;
-    for (int p = 0; p < n_pat; ++p) {
-        const mpb_pattern pt = pats[p];
-        if (x + pt.len > n_col) continue;
-        uint32_t acc = 0xFFFFFFFFu;
-        for (int i = 0; i < pt.len && acc; ++i) {
-            uint32_t m = 0;
-#pragma unroll
-            for (int b = 0; b < 4; ++b)
-                if ((pt.allow[b] >> i) & 1u) m |= __ldg(colp + ((long long)(x + i) * 4 + b) * nwords + w);
-            acc &= m;
-        }
-        while (acc) {
-            const int bit = __ffs(acc) - 1;
-            acc &= acc - 1;
-            const unsigned long long slot = atomicAdd(n_hits, 1ull);
-            if ((long long)slot < max_hits) {
-                hit_pat[slot] = p;
-                hit_row[slot] = (int32_t)(w * 32 + bit);
-                hit_pos[slot] = x;
+    for (int x = blockIdx.y; x < n_col; x += gridDim.y) {
+        for (int p = 0; p < n_pat; ++p) {
+            const mpb_pattern pt = pats[p];
+            if (x + pt.len > n_col) continue;
+            uint32_t acc = 0xFFFFFFFFu;
+            for (int i = 0; i < pt.len && acc; ++i) {
+                const uint32_t* c = colp + (long long)(x + i) * 4 * nwords + w;
+                const uint32_t pa = __ldg(c), pc = __ldg(c + nwords), pg = __ldg(c + 2 * nwords), pt4 = __ldg(c + 3 * nwords);
+                const uint32_t multi = ((pa | pc) & (pg | pt4)) | (pa & pc) | (pg & pt4);  // two or more planes set
+                uint32_t m = 0;
+                if ((pt.allow[0] >> i) & 1u) m |= pa;
+                if ((pt.allow[1] >> i) & 1u) m |= pc;
+                if ((pt.allow[2] >> i) & 1u) m |= pg;
+                if ((pt.allow[3] >> i) & 1u) m |= pt4;
+                acc &= m & ~multi;
+            }
+            while (acc) {
+                const int bit = __ffs(acc) - 1;
+                acc &= acc - 1;
+                const unsigned long long slot = atomicAdd(n_hits, 1ull);
+                if ((long long)slot < max_hits) {
+                    hit_pat[slot] = p;
+                    hit_row[slot] = (int32_t)(w * 32 + bit);
+                    hit_pos[slot] = x;
+                }
             }
         }
     }
@@ -454,7 +464,8 @@ extern "C" int mpb_pattern_hits(mpb_msa* m, int32_t n_pat, const uint32_t* allow
     CK(cudaMallocAsync(&dn, 8, ctx->stream));
     CK(cudaMemsetAsync(dn, 0, 8, ctx->stream));
     ctx->pending_units = (double)n_pat * (double)m->n_seq * (double)m->n_col;
-    LAUNCH(ctx, k_pattern_hits, dim3((unsigned)((m->nwords + 255) / 256), (unsigned)m->n_col), 256, 0, m->colp,
+    const unsigned gy = (unsigned)(m->n_col < PATTERN_MAX_GY ? m->n_col : PATTERN_MAX_GY);
+    LAUNCH(ctx, k_pattern_hits, dim3((unsigned)((m->nwords + 255) / 256), gy), 256, 0, m->colp,
            (long long)m->nwords, (int)m->n_col, pd.dev<mpb_pattern>(), (int)n_pat, (long long)max_hits, op.dev<int32_t>(),
            orow.dev<int32_t>(), opos.dev<int32_t>(), dn);
     unsigned long long n = 0;
