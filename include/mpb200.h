@@ -208,6 +208,15 @@ int mpb_cscan(mpb_hist* h, uint32_t fmask, uint32_t rmask, const mpb_cand* cands
 int mpb_pattern_hits(mpb_msa* msa, int32_t n_pat, const uint32_t* allow, const int32_t* lens, int64_t max_hits,
                      int32_t* hit_pat, int32_t* hit_row, int32_t* hit_pos, int64_t* n_hits);
 
+/* The same search with up to v mismatches per site (primer_coverage.py, the mismatch rule of mis_primer_check
+ * core:1103-1130): a site of pattern p at position x of a row is reported when the pattern lies inside the row's lens,
+ * at most v of its cells mismatch (a cell that is not exactly one allowed base mismatches) and none of the mismatches
+ * falls on a position whose bit is set in strict[p] (host array).  hit_mis receives the site's mismatch count; the other
+ * outputs and the capacity rule are those of mpb_pattern_hits.  0 <= v <= 15 and v < lens[p] for every pattern. */
+int mpb_pattern_sites(mpb_msa* msa, int32_t n_pat, const uint32_t* allow, const int32_t* lens, const uint32_t* strict,
+                      int32_t v, int64_t max_hits, int32_t* hit_pat, int32_t* hit_row, int32_t* hit_pos, int32_t* hit_mis,
+                      int64_t* n_hits);
+
 /* Per (window, sequence) haplotype key, for the JSON side files (core:1172-1176): the table key of the
  * sequence's k-mer, MPB_KEY_IUPAC for rows whose window holds IUPAC cells. out[nw*n_seq]. */
 #define MPB_KEY_IUPAC 0xFFFFFFFFFFFFFFFEull

@@ -52,6 +52,8 @@ SIGNATURES = {
     "mpb_hist_exceptions": (C.c_int, [_P, C.c_int64, _P, _P, C.POINTER(C.c_int64)]),
     "mpb_scan": (C.c_int, [_P, C.c_int, C.c_int, C.c_uint32, C.c_uint32, _P, _P, C.c_int64, _P, _P, _P]),
     "mpb_pattern_hits": (C.c_int, [_P, C.c_int32, _P, _P, C.c_int64, _P, _P, _P, C.POINTER(C.c_int64)]),
+    "mpb_pattern_sites": (C.c_int, [_P, C.c_int32, _P, _P, _P, C.c_int32, C.c_int64, _P, _P, _P, _P,
+                                    C.POINTER(C.c_int64)]),
     "mpb_seqkeys": (C.c_int, [_P, C.c_int, _P, C.c_int32, _P]),
     "mpb_tm": (C.c_int, [_P, _P, C.c_int, C.c_int64, _P, _P, _P, _P]),
     "mpb_tm_sets": (C.c_int, [_P, _P, C.c_int, C.c_int32, _P, _P, _P]),
@@ -436,6 +438,24 @@ class Msa:
         n = n.value
         order = np.lexsort((hx[:n], hr[:n], hp[:n]))
         return hp[:n][order], hr[:n][order], hx[:n][order]
+
+    def pattern_sites(self, allow, lens, strict, v: int, max_hits: int = 1 << 20):
+        """mpb_pattern_sites: every site of the degenerate patterns with at most v mismatches and none at a strict
+        position -> (pattern, sequence, position, mismatches) arrays sorted by (pattern, sequence, position)"""
+        allow = np.ascontiguousarray(allow, dtype=np.uint32).reshape(-1, 4)
+        lens = np.ascontiguousarray(lens, dtype=np.int32)
+        strict = np.ascontiguousarray(strict, dtype=np.uint32)
+        while True:
+            hp, hr, hx, hm = (np.empty(max_hits, np.int32) for _ in range(4))
+            n = C.c_int64()
+            check(load().mpb_pattern_sites(self.h, len(lens), ptr(allow), ptr(lens), ptr(strict), v, max_hits, ptr(hp),
+                                           ptr(hr), ptr(hx), ptr(hm), C.byref(n)))
+            if n.value <= max_hits:
+                break
+            max_hits = int(n.value) + 16
+        n = n.value
+        order = np.lexsort((hx[:n], hr[:n], hp[:n]))
+        return hp[:n][order], hr[:n][order], hx[:n][order], hm[:n][order]
 
     def seqkeys(self, k: int, win_pos) -> np.ndarray:
         win_pos = np.ascontiguousarray(win_pos, dtype=np.int32)

@@ -394,24 +394,32 @@ extern "C" int mpb_cscan(mpb_hist* h, uint32_t fmask, uint32_t rmask, const mpb_
 }
 
 // ---- exhaustive pattern search (SURVEY.md 8f-4) -----------------------------------------------------------------------
-// Every position of every sequence against a set of degenerate patterns, exact match: the in-silico PCR of
-// extract_PCR_product_V1.py:189-216 (and the coverage validation the pipeline otherwise delegates to bowtie2) asks "where
-// does an expansion of this primer occur in this sequence".  On the column view that is the scan kernel with the window
-// start as a free variable: thread = (position, 32-sequence word); the running AND of the per-column match words dies
-// after two or three columns almost everywhere.  Hits are rare and leave as (pattern, sequence, position) triples.
-// A cell matches only when it holds exactly one base and that base is allowed: an IUPAC cell sets two or more planes
-// and the reference's plain-text search never matches it.  Columns are walked with stride gridDim.y (capped at 65535),
-// so lines of any width fit one launch.
+// Every position of every sequence against a set of degenerate patterns: the in-silico PCR of
+// extract_PCR_product_V1.py:189-216 and primer_coverage.py asks "where does an expansion of this primer occur (with at
+// most v mismatches) in this sequence".  On the column view that is the scan kernel with the window start as a free
+// variable: thread = (position, 32-sequence word).  Sites are rare and leave as (pattern, sequence, position[,
+// mismatches]) tuples.  A cell matches only when it holds exactly one base and that base is allowed: an IUPAC cell sets
+// two or more planes and the reference's plain-text search never matches it.  Columns are walked with stride gridDim.y
+// (capped at 65535), so lines of any width fit one launch.
+//   NB == 0  exact search (mpb_pattern_hits): the running AND of the per-column match words dies after two or three
+//            columns almost everywhere.
+//   NB > 0   mismatch-bounded search (mpb_pattern_sites): per-lane mismatch counts in NB bit-sliced saturating words (the
+//            Counter of k_cscan), the mismatch words of the strict positions ORed into a "dead" word; a lane stops when
+//            it is dead or over v, so on random sequence the walk ends after about v + 2 columns.  Cells past a row's
+//            length are zero (no base) and no longer rule a site out, so emitted sites are checked against lens.
 struct mpb_pattern {
     uint32_t allow[4];
     int32_t len;
+    uint32_t strict;  // positions where a mismatch disqualifies the site (NB > 0 only)
 };
 
 #define PATTERN_MAX_GY 65535
 
+template <int NB>
 __global__ void __launch_bounds__(256)
 k_pattern_hits(const uint32_t* __restrict__ colp, long long nwords, int n_col, const mpb_pattern* __restrict__ pats, int n_pat,
-               long long max_hits, int32_t* __restrict__ hit_pat, int32_t* __restrict__ hit_row, int32_t* __restrict__ hit_pos,
+               int v, long long n_seq, const int32_t* __restrict__ lens, long long max_hits, int32_t* __restrict__ hit_pat,
+               int32_t* __restrict__ hit_row, int32_t* __restrict__ hit_pos, int32_t* __restrict__ hit_mis,
                unsigned long long* __restrict__ n_hits) {
     const long long w = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (w >= nwords) return;
@@ -419,7 +427,10 @@ k_pattern_hits(const uint32_t* __restrict__ colp, long long nwords, int n_col, c
         for (int p = 0; p < n_pat; ++p) {
             const mpb_pattern pt = pats[p];
             if (x + pt.len > n_col) continue;
-            uint32_t acc = 0xFFFFFFFFu;
+            uint32_t acc = 0xFFFFFFFFu;  // NB == 0: lanes still matching; NB > 0: lanes neither dead nor over v
+            Counter<NB == 0 ? 1 : NB> cnt;
+            cnt.clear();
+            uint32_t dead = 0;
             for (int i = 0; i < pt.len && acc; ++i) {
                 const uint32_t* c = colp + (long long)(x + i) * 4 * nwords + w;
                 const uint32_t pa = __ldg(c), pc = __ldg(c + nwords), pg = __ldg(c + 2 * nwords), pt4 = __ldg(c + 3 * nwords);
@@ -429,53 +440,96 @@ k_pattern_hits(const uint32_t* __restrict__ colp, long long nwords, int n_col, c
                 if ((pt.allow[1] >> i) & 1u) m |= pc;
                 if ((pt.allow[2] >> i) & 1u) m |= pg;
                 if ((pt.allow[3] >> i) & 1u) m |= pt4;
-                acc &= m & ~multi;
+                if (NB == 0) {
+                    acc &= m & ~multi;
+                } else {
+                    const uint32_t mis = ~(m & ~multi);
+                    if ((pt.strict >> i) & 1u) dead |= mis;
+                    cnt.add(mis, 0);
+                    acc = ~(dead | cnt.over(v));
+                }
             }
             while (acc) {
                 const int bit = __ffs(acc) - 1;
                 acc &= acc - 1;
+                const long long row = w * 32 + bit;
+                if (NB > 0 && (row >= n_seq || x + pt.len > __ldg(lens + row))) continue;
                 const unsigned long long slot = atomicAdd(n_hits, 1ull);
                 if ((long long)slot < max_hits) {
                     hit_pat[slot] = p;
-                    hit_row[slot] = (int32_t)(w * 32 + bit);
+                    hit_row[slot] = (int32_t)row;
                     hit_pos[slot] = x;
+                    if (NB > 0) {
+                        int nm = 0;
+#pragma unroll
+                        for (int b = 0; b < (NB == 0 ? 1 : NB); ++b) nm |= (int)((cnt.b[b] >> bit) & 1u) << b;
+                        hit_mis[slot] = nm;
+                    }
                 }
             }
         }
     }
 }
 
-extern "C" int mpb_pattern_hits(mpb_msa* m, int32_t n_pat, const uint32_t* allow, const int32_t* lens, int64_t max_hits,
-                                int32_t* hit_pat, int32_t* hit_row, int32_t* hit_pos, int64_t* n_hits) {
+// v < 0: exact search (mpb_pattern_hits; strict and hit_mis unused)
+static int pattern_search(mpb_msa* m, int32_t n_pat, const uint32_t* allow, const int32_t* lens, const uint32_t* strict,
+                          int v, int64_t max_hits, int32_t* hit_pat, int32_t* hit_row, int32_t* hit_pos, int32_t* hit_mis,
+                          int64_t* n_hits) {
     if (!m || !allow || !lens || !hit_pat || !hit_row || !hit_pos || !n_hits) return fail(MPB_EINVAL, "NULL argument");
+    if (v >= 0 && (!strict || !hit_mis)) return fail(MPB_EINVAL, "NULL argument");
     if (n_pat < 1 || max_hits < 0) return fail(MPB_EINVAL, "bad n_pat or max_hits");
+    if (v > 15) return fail(MPB_EINVAL, "at most 15 mismatches are supported (got %d)", v);
     mpb_ctx* ctx = m->ctx;
     CK(cudaSetDevice(ctx->device));
     std::vector<mpb_pattern> pats(n_pat);
     for (int i = 0; i < n_pat; ++i) {
         if (lens[i] < 1 || lens[i] > 32) return fail(MPB_EINVAL, "pattern %d: length %d outside 1..32", i, lens[i]);
+        if (v >= lens[i])
+            return fail(MPB_EINVAL, "pattern %d: %d mismatches allowed on a %d-base pattern match everywhere", i, v, lens[i]);
         for (int b = 0; b < 4; ++b) pats[i].allow[b] = allow[i * 4 + b];
         pats[i].len = lens[i];
+        pats[i].strict = v >= 0 ? strict[i] : 0u;
     }
     InBuf pd(ctx, pats.data(), pats.size() * sizeof(mpb_pattern));
-    OutBuf op(ctx, hit_pat, (size_t)max_hits * 4), orow(ctx, hit_row, (size_t)max_hits * 4), opos(ctx, hit_pos, (size_t)max_hits * 4);
-    if (pd.rc || op.rc || orow.rc || opos.rc) return MPB_ECUDA;
+    OutBuf op(ctx, hit_pat, (size_t)max_hits * 4), orow(ctx, hit_row, (size_t)max_hits * 4), opos(ctx, hit_pos, (size_t)max_hits * 4),
+        omis(ctx, v >= 0 ? hit_mis : nullptr, v >= 0 ? (size_t)max_hits * 4 : 0);
+    if (pd.rc || op.rc || orow.rc || opos.rc || omis.rc) return MPB_ECUDA;
     unsigned long long* dn = nullptr;
     CK(cudaMallocAsync(&dn, 8, ctx->stream));
     CK(cudaMemsetAsync(dn, 0, 8, ctx->stream));
     ctx->pending_units = (double)n_pat * (double)m->n_seq * (double)m->n_col;
     const unsigned gy = (unsigned)(m->n_col < PATTERN_MAX_GY ? m->n_col : PATTERN_MAX_GY);
-    LAUNCH(ctx, k_pattern_hits, dim3((unsigned)((m->nwords + 255) / 256), gy), 256, 0, m->colp,
-           (long long)m->nwords, (int)m->n_col, pd.dev<mpb_pattern>(), (int)n_pat, (long long)max_hits, op.dev<int32_t>(),
-           orow.dev<int32_t>(), opos.dev<int32_t>(), dn);
+    const dim3 grid((unsigned)((m->nwords + 255) / 256), gy);
+#define PATTERN_ARGS                                                                                                       \
+    m->colp, (long long)m->nwords, (int)m->n_col, pd.dev<mpb_pattern>(), (int)n_pat, v, (long long)m->n_seq, m->lens,      \
+        (long long)max_hits, op.dev<int32_t>(), orow.dev<int32_t>(), opos.dev<int32_t>(), omis.dev<int32_t>(), dn
+    if (v < 0)
+        MPB_LAUNCH_NAMED(ctx, "k_pattern_hits", k_pattern_hits<0>, grid, 256, 0, PATTERN_ARGS);
+    else if (v <= 3)
+        MPB_LAUNCH_NAMED(ctx, "k_pattern_sites", k_pattern_hits<3>, grid, 256, 0, PATTERN_ARGS);
+    else
+        MPB_LAUNCH_NAMED(ctx, "k_pattern_sites", k_pattern_hits<5>, grid, 256, 0, PATTERN_ARGS);
+#undef PATTERN_ARGS
     unsigned long long n = 0;
     CK(cudaMemcpyAsync(&n, dn, 8, cudaMemcpyDeviceToHost, ctx->stream));
     CK(op.finish());
     CK(orow.finish());
     CK(opos.finish());
+    CK(omis.finish());
     CK(cudaStreamSynchronize(ctx->stream));
     CK(cudaFreeAsync(dn, ctx->stream));
     *n_hits = (int64_t)n;
     return 0;
 }
 
+extern "C" int mpb_pattern_hits(mpb_msa* m, int32_t n_pat, const uint32_t* allow, const int32_t* lens, int64_t max_hits,
+                                int32_t* hit_pat, int32_t* hit_row, int32_t* hit_pos, int64_t* n_hits) {
+    return pattern_search(m, n_pat, allow, lens, nullptr, -1, max_hits, hit_pat, hit_row, hit_pos, nullptr, n_hits);
+}
+
+extern "C" int mpb_pattern_sites(mpb_msa* m, int32_t n_pat, const uint32_t* allow, const int32_t* lens,
+                                 const uint32_t* strict, int32_t v, int64_t max_hits, int32_t* hit_pat, int32_t* hit_row,
+                                 int32_t* hit_pos, int32_t* hit_mis, int64_t* n_hits) {
+    if (v < 0) return fail(MPB_EINVAL, "negative mismatch bound %d", v);
+    return pattern_search(m, n_pat, allow, lens, strict, v, max_hits, hit_pat, hit_row, hit_pos, hit_mis, n_hits);
+}

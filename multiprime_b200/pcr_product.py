@@ -86,6 +86,37 @@ def allow_of(primer: str):
     return allow
 
 
+def parse_primers(primer_file, file_format):
+    """extract_PCR_product_V1.py:141-167: {pair name: [primer_F, primer_R]} from a final_maxprimers_set.xls (xls), a
+    four-line-per-pair FASTA (fa) or "F,R" (seq)"""
+    res = {}
+    if file_format == "seq":
+        primers = primer_file.split(",")
+        res["PCR_info"] = [primers[0], primers[1]]
+        return res
+    with open(primer_file, "r") as f:
+        if file_format == "xls":
+            for line in f:
+                if line.startswith("#"):
+                    continue
+                i = line.strip().split("\t")
+                cluster_id = i[0].split("/")[-1].split(".")[0]
+                start, stop = i[6].split(":")[0], i[6].split(":")[1]
+                res[cluster_id + "_" + str(start) + "_F_" + cluster_id + "_" + str(stop)] = [i[2], i[3]]
+        elif file_format == "fa":
+            rows = [ln.rstrip("\n") for ln in f if ln.strip() != ""]      # pandas.read_table skips blank lines
+            for idx, row in enumerate(rows):
+                if idx % 4 == 0:
+                    primer_f_info = row.lstrip(">")
+                elif idx % 4 == 1:
+                    primer_f = row
+                elif idx % 4 == 2:
+                    key = primer_f_info + "_" + row.lstrip(">")
+                else:
+                    res[key] = [primer_f, row]
+    return res
+
+
 class Product(object):
     """extract_PCR_product_V1.py:123-133 constructor arguments"""
 
@@ -103,32 +134,7 @@ class Product(object):
 
     def parse_primers(self):
         """extract_PCR_product_V1.py:141-167"""
-        res = {}
-        if self.file_format == "seq":
-            primers = self.primers_file.split(",")
-            res["PCR_info"] = [primers[0], primers[1]]
-            return res
-        with open(self.primers_file, "r") as f:
-            if self.file_format == "xls":
-                for line in f:
-                    if line.startswith("#"):
-                        continue
-                    i = line.strip().split("\t")
-                    cluster_id = i[0].split("/")[-1].split(".")[0]
-                    start, stop = i[6].split(":")[0], i[6].split(":")[1]
-                    res[cluster_id + "_" + str(start) + "_F_" + cluster_id + "_" + str(stop)] = [i[2], i[3]]
-            elif self.file_format == "fa":
-                rows = [ln.rstrip("\n") for ln in f if ln.strip() != ""]      # pandas.read_table skips blank lines
-                for idx, row in enumerate(rows):
-                    if idx % 4 == 0:
-                        primer_f_info = row.lstrip(">")
-                    elif idx % 4 == 1:
-                        primer_f = row
-                    elif idx % 4 == 2:
-                        key = primer_f_info + "_" + row.lstrip(">")
-                    else:
-                        res[key] = [primer_f, row]
-        return res
+        return parse_primers(self.primers_file, self.file_format)
 
     # -- device part ----------------------------------------------------------------------------------------
     def _hits(self, lines):

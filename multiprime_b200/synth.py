@@ -110,3 +110,52 @@ def write_fasta(path: str, codes: np.ndarray, row0: int = 0) -> None:
     with open(path, "w") as fh:
         for sid, s in zip(seq_ids(len(codes), row0), codes_to_strings(codes)):
             fh.write(sid + "\n" + s + "\n")
+
+
+_COMP = np.array([3, 2, 1, 0], np.uint8)          # base index (A,C,G,T) -> complement
+
+
+def write_pcr_targets(path: str, n_targets: int = 65536, length: int = 10_000, n_pairs: int = 48, seed: int = 20241015):
+    """The in-silico PCR workload (tools/bench_pcr.py): a FASTA of n_targets unaligned targets of about `length`
+    bases from a clade-structured root — 8 clades with their own substitutions, 1 % point mutations, a few short indels,
+    random trims of up to 200 bases at each end, half of the targets reverse-complemented — and n_pairs primer pairs
+    (20-mers) cut from the root, a third of them with one or two degenerate positions.  Returns {name: (F, R)}."""
+    rng = np.random.Generator(np.random.PCG64([seed, 0x9C2]))
+    root = rng.integers(0, 4, length).astype(np.uint8)
+    clade_cols = rng.choice(length, (8, 40))
+    clade_shift = rng.integers(1, 4, (8, 40)).astype(np.uint8)
+    letters = np.frombuffer(b"ACGT", np.uint8)
+    pairs = {}
+    starts = np.sort(rng.choice(np.arange(100, length - 1700), n_pairs, replace=False))
+    for q, a in enumerate(starts.tolist()):
+        b = a + int(rng.integers(200, 1500))
+        f = ["ACGT"[x] for x in root[a:a + 20]]
+        r = ["ACGT"[3 - x] for x in root[b:b + 20][::-1]]
+        if q % 3 == 0:
+            for p in rng.choice(np.arange(3, 17), int(rng.integers(1, 3)), replace=False):
+                f[p] = {"A": "R", "G": "R", "C": "Y", "T": "Y"}[f[p]]
+        pairs["pair%02d" % q] = ("".join(f), "".join(r))
+    chunk = 4096
+    with open(path, "wb") as fh:
+        for c0 in range(0, n_targets, chunk):
+            n = min(chunk, n_targets - c0)
+            x = np.broadcast_to(root, (n, length)).copy()
+            clade = rng.integers(0, 8, n)
+            for k in range(8):
+                rows = np.nonzero(clade == k)[0]
+                x[np.ix_(rows, clade_cols[k])] = (x[np.ix_(rows, clade_cols[k])] + clade_shift[k]) % 4
+            mut = rng.random((n, length), dtype=np.float32) < 0.01
+            x = np.where(mut, (x + rng.integers(1, 4, (n, length), dtype=np.uint8)) % 4, x).astype(np.uint8)
+            out = []
+            for i in range(n):
+                s = x[i]
+                for _ in range(int(rng.poisson(2))):
+                    p, d = int(rng.integers(0, len(s) - 8)), int(rng.integers(1, 6))
+                    s = np.delete(s, np.arange(p, p + d)) if rng.random() < 0.5 else \
+                        np.insert(s, p, rng.integers(0, 4, d).astype(np.uint8))
+                s = s[int(rng.integers(0, 200)):len(s) - int(rng.integers(0, 200))]
+                if (c0 + i) % 2:
+                    s = _COMP[s[::-1]]
+                out.append(b">t%07d\n" % (c0 + i) + letters[s].tobytes() + b"\n")
+            fh.write(b"".join(out))
+    return pairs
