@@ -217,6 +217,29 @@ int mpb_pattern_sites(mpb_msa* msa, int32_t n_pat, const uint32_t* allow, const 
                       int32_t v, int64_t max_hits, int32_t* hit_pat, int32_t* hit_row, int32_t* hit_pos, int32_t* hit_mis,
                       int64_t* n_hits);
 
+/* In-silico PCR over every primer combination (primer_specificity.py).  The handle's rows are overlapping cuts of one
+ * stream: row r holds stream columns [r*stride, r*stride + n_col).  The patterns (allow / lens / strict / v as in
+ * mpb_pattern_sites) belong to primers: pattern p is a LEFT site of primer pat_primer[p] (pat_side[p] == 0: the primer
+ * binds on the stored strand) or a RIGHT site (1: its reverse complement binds).  A site is kept when it starts in the
+ * first `stride` columns of its row and lies inside one of the n_rec records (stream offsets rec_off[] ascending and
+ * lengths rec_len[], relative to row 0 of the handle).  A product (i, j) is a left site of i at x and a right site of j
+ * at y in one record with y >= x + L_i and y + L_j - x in [lo, hi]; a group is (record, i, j) with at least one
+ * product, and its best product has the fewest total mismatches, then the smallest length, then the smallest x.
+ * Sites, products and groups stay on the device; memory is bounded by sites + groups (left sites are joined in chunks
+ * of at most `chunk`, 0 = default).  Host outputs:
+ *   comb[(i*n_primer + j)*3 + {0,1,2}]  products, groups (targets), groups whose best product has no mismatch;
+ *   uni[2]   records with a group of a combination whose list[i*n_primer + j] is set, and those with a perfect one;
+ *   rows[max_rows*8]  the first max_rows listed groups in (record, i, j) order: record, i, j, start, length, left
+ *            mismatches, right mismatches, products (start 0-based on the record); *n_listed = all listed groups;
+ *   stats[4] search hits, left sites, right sites, groups.
+ * Limits (MPB_EINVAL): 1 <= n_primer <= 1024, 0 < lo <= hi <= 2^23 - 1, records shorter than 2^32, a stream shorter
+ * than 2^43 columns. */
+int mpb_pattern_products(mpb_msa* msa, int32_t n_pat, const uint32_t* allow, const int32_t* lens, const uint32_t* strict,
+                         int32_t v, const int32_t* pat_primer, const int32_t* pat_side, int32_t n_primer, int64_t stride,
+                         int32_t n_rec, const int64_t* rec_off, const int64_t* rec_len, int32_t lo, int32_t hi,
+                         const uint8_t* list, int64_t chunk, int64_t max_rows, int64_t* comb, int64_t* uni, int64_t* rows,
+                         int64_t* n_listed, int64_t* stats);
+
 /* Per (window, sequence) haplotype key, for the JSON side files (core:1172-1176): the table key of the
  * sequence's k-mer, MPB_KEY_IUPAC for rows whose window holds IUPAC cells. out[nw*n_seq]. */
 #define MPB_KEY_IUPAC 0xFFFFFFFFFFFFFFFEull

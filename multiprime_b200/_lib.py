@@ -54,6 +54,9 @@ SIGNATURES = {
     "mpb_pattern_hits": (C.c_int, [_P, C.c_int32, _P, _P, C.c_int64, _P, _P, _P, C.POINTER(C.c_int64)]),
     "mpb_pattern_sites": (C.c_int, [_P, C.c_int32, _P, _P, _P, C.c_int32, C.c_int64, _P, _P, _P, _P,
                                     C.POINTER(C.c_int64)]),
+    "mpb_pattern_products": (C.c_int, [_P, C.c_int32, _P, _P, _P, C.c_int32, _P, _P, C.c_int32, C.c_int64, C.c_int32,
+                                       _P, _P, C.c_int32, C.c_int32, _P, C.c_int64, C.c_int64, _P, _P, _P,
+                                       C.POINTER(C.c_int64), _P]),
     "mpb_seqkeys": (C.c_int, [_P, C.c_int, _P, C.c_int32, _P]),
     "mpb_tm": (C.c_int, [_P, _P, C.c_int, C.c_int64, _P, _P, _P, _P]),
     "mpb_tm_sets": (C.c_int, [_P, _P, C.c_int, C.c_int32, _P, _P, _P]),
@@ -456,6 +459,32 @@ class Msa:
         n = n.value
         order = np.lexsort((hx[:n], hr[:n], hp[:n]))
         return hp[:n][order], hr[:n][order], hx[:n][order], hm[:n][order]
+
+    def pattern_products(self, allow, lens, strict, v: int, pat_primer, pat_side, n_primer: int, stride: int, rec_off,
+                         rec_len, lo: int, hi: int, listed, max_rows: int, chunk: int = 0):
+        """mpb_pattern_products: products of every (left primer i, right primer j) combination in the records, joined on
+        the device -> dict(comb int64[n_primer, n_primer, 3] (products, targets, perfect targets), union int64[2]
+        (targets and perfect targets over the combinations flagged in listed[n_primer, n_primer]), rows int64[n, 8]
+        (the first max_rows listed groups: record, i, j, start, length, left / right mismatches, products), n_listed,
+        stats int64[4] (search hits, left sites, right sites, groups))"""
+        allow = np.ascontiguousarray(allow, dtype=np.uint32).reshape(-1, 4)
+        lens = np.ascontiguousarray(lens, dtype=np.int32)
+        strict = np.ascontiguousarray(strict, dtype=np.uint32)
+        pat_primer = np.ascontiguousarray(pat_primer, dtype=np.int32)
+        pat_side = np.ascontiguousarray(pat_side, dtype=np.int32)
+        rec_off = np.ascontiguousarray(rec_off, dtype=np.int64)
+        rec_len = np.ascontiguousarray(rec_len, dtype=np.int64)
+        listed = np.ascontiguousarray(listed, dtype=np.uint8).reshape(n_primer, n_primer)
+        comb = np.zeros((n_primer, n_primer, 3), np.int64)
+        uni = np.zeros(2, np.int64)
+        rows = np.zeros((max(max_rows, 1), 8), np.int64)
+        stats = np.zeros(4, np.int64)
+        n = C.c_int64()
+        check(load().mpb_pattern_products(self.h, len(lens), ptr(allow), ptr(lens), ptr(strict), v, ptr(pat_primer),
+                                          ptr(pat_side), n_primer, stride, len(rec_off), ptr(rec_off), ptr(rec_len), lo,
+                                          hi, ptr(listed), chunk, max_rows, ptr(comb), ptr(uni), ptr(rows), C.byref(n),
+                                          ptr(stats)))
+        return dict(comb=comb, union=uni, rows=rows[:min(n.value, max_rows)], n_listed=n.value, stats=stats)
 
     def seqkeys(self, k: int, win_pos) -> np.ndarray:
         win_pos = np.ascontiguousarray(win_pos, dtype=np.int32)

@@ -472,9 +472,9 @@ k_pattern_hits(const uint32_t* __restrict__ colp, long long nwords, int n_col, c
 }
 
 // v < 0: exact search (mpb_pattern_hits; strict and hit_mis unused)
-static int pattern_search(mpb_msa* m, int32_t n_pat, const uint32_t* allow, const int32_t* lens, const uint32_t* strict,
-                          int v, int64_t max_hits, int32_t* hit_pat, int32_t* hit_row, int32_t* hit_pos, int32_t* hit_mis,
-                          int64_t* n_hits) {
+int mpb_pattern_search(mpb_msa* m, int32_t n_pat, const uint32_t* allow, const int32_t* lens, const uint32_t* strict,
+                       int v, int64_t max_hits, int32_t* hit_pat, int32_t* hit_row, int32_t* hit_pos, int32_t* hit_mis,
+                       int64_t* n_hits) {
     if (!m || !allow || !lens || !hit_pat || !hit_row || !hit_pos || !n_hits) return fail(MPB_EINVAL, "NULL argument");
     if (v >= 0 && (!strict || !hit_mis)) return fail(MPB_EINVAL, "NULL argument");
     if (n_pat < 1 || max_hits < 0) return fail(MPB_EINVAL, "bad n_pat or max_hits");
@@ -524,12 +524,12 @@ static int pattern_search(mpb_msa* m, int32_t n_pat, const uint32_t* allow, cons
 
 extern "C" int mpb_pattern_hits(mpb_msa* m, int32_t n_pat, const uint32_t* allow, const int32_t* lens, int64_t max_hits,
                                 int32_t* hit_pat, int32_t* hit_row, int32_t* hit_pos, int64_t* n_hits) {
-    return pattern_search(m, n_pat, allow, lens, nullptr, -1, max_hits, hit_pat, hit_row, hit_pos, nullptr, n_hits);
+    return mpb_pattern_search(m, n_pat, allow, lens, nullptr, -1, max_hits, hit_pat, hit_row, hit_pos, nullptr, n_hits);
 }
 
 extern "C" int mpb_pattern_sites(mpb_msa* m, int32_t n_pat, const uint32_t* allow, const int32_t* lens,
                                  const uint32_t* strict, int32_t v, int64_t max_hits, int32_t* hit_pat, int32_t* hit_row,
                                  int32_t* hit_pos, int32_t* hit_mis, int64_t* n_hits) {
     if (v < 0) return fail(MPB_EINVAL, "negative mismatch bound %d", v);
-    return pattern_search(m, n_pat, allow, lens, strict, v, max_hits, hit_pat, hit_row, hit_pos, hit_mis, n_hits);
+    return mpb_pattern_search(m, n_pat, allow, lens, strict, v, max_hits, hit_pat, hit_row, hit_pos, hit_mis, n_hits);
 }

@@ -16,3 +16,10 @@
 int mpb_cscan_launch(mpb_hist* h, uint32_t fmask, uint32_t rmask, const mpb_cand* cands_d, const int* n_cand_d,
                      int max_cands, uint32_t* plans_d, unsigned long long* counts_d, int zero_counts,
                      const int32_t* bits_slot_d, uint32_t* bits_d, int plans_ready);
+
+// The exhaustive pattern search behind mpb_pattern_hits (v < 0) and mpb_pattern_sites (v >= 0).  The hit outputs may be
+// host or device memory (device: they stay there, as mpb_pattern_products needs); *n_hits may exceed max_hits.
+// Synchronises the context's stream.
+int mpb_pattern_search(mpb_msa* m, int32_t n_pat, const uint32_t* allow, const int32_t* lens, const uint32_t* strict,
+                       int v, int64_t max_hits, int32_t* hit_pat, int32_t* hit_row, int32_t* hit_pos, int32_t* hit_mis,
+                       int64_t* n_hits);
