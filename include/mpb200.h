@@ -98,6 +98,9 @@ int mpb_seq_attr_hist(mpb_msa* msa, int64_t* lead_hist_hd, int64_t* rstrip_hist_
  * For every window start win_pos[i] (host array) extract each sequence's k-mer with the reference's
  * terminal-gap patching, expand IUPAC cells, and count haplotypes into an open-addressing table per window
  * (cover / gap_sequence dictionaries of the reference).  log2_cap = 0 picks 2^ceil(log2(2*n_seq+64)).
+ * Any start 0 <= win_pos[i] < n_col is accepted.  A window with win_pos[i] + k > n_col (or past a ragged row's end)
+ * takes the reference's left extension (core:683-687): the row's cells from win_pos[i] on, patched, preceded by the
+ * bases left of them; a row without enough bases there fails the call with MPB_EEXPAND.
  */
 int mpb_hist_build(mpb_msa* msa, int k, int v, const int32_t* win_pos, int32_t nw, int log2_cap, mpb_hist** out);
 void mpb_hist_free(mpb_hist* h);

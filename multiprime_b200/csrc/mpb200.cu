@@ -1362,6 +1362,11 @@ static int hist_launch_build(mpb_hist* h) {
     CK(cudaMemsetAsync(h->spec_n, 0, (size_t)nw * 8, ctx->stream));
     CK(cudaMemsetAsync(h->exc_n, 0, 8, ctx->stream));
     if (mpb_use_col_passes()) {
+        // A window that runs past the last column takes the reference's left extension (core:683-687) on every row.
+        // The column view reads the missing cells as gaps, so such a batch flags its rows like those of a ragged input
+        // (lens = n_col): col_ragged marks the rows of those windows special, and hist_row cuts them.
+        bool ragged = m->short_rows;
+        for (int i = 0; i < nw; ++i) ragged = ragged || h->h_win_pos[i] + h->k > m->n_col;
         std::vector<int2> chunks;
         std::vector<int32_t> chunk_win;
         mpb_window_chunks(h->h_win_pos.data(), nw, h->k, chunks, chunk_win);
@@ -1391,7 +1396,7 @@ static int hist_launch_build(mpb_hist* h) {
         ctx->pending_units = (double)nw * (double)m->n_seq;
         MPB_LAUNCH_NAMED(ctx, "k_hist", k_hist_col, dim3(gx, (unsigned)chunks.size()), CW_THREADS, 0, m->colp, (m->ncw - 1) * 32,
                          m->cons, m->planes, m->nsp, m->n_seq, m->lens, h->k, h->v, h->win_pos, cd.dev<int2>(),
-                         cw.dev<int32_t>(), (int)chunks.size(), o, m->short_rows ? 1 : 0, m->err);
+                         cw.dev<int32_t>(), (int)chunks.size(), o, ragged ? 1 : 0, m->err);
         return 0;
     }
     const unsigned gx = (unsigned)((m->n_seq + (long long)WIN_ROWS - 1) / (long long)WIN_ROWS);
