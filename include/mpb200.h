@@ -390,6 +390,15 @@ int mpb_dimer_pairs(mpb_dimer* d, const int32_t* pi, const int32_t* pj, int64_t 
 int mpb_dimer_grid(mpb_dimer* d, int32_t row0, int32_t row1, int64_t max_hits, int32_t* hit_i, int32_t* hit_j,
                    int64_t* hit_order, int32_t* hit_d2, int64_t* n_hits, int64_t* n_tested);
 
+/* ---- pool assignment: multiprime_b200/primer_pools.py states the search rule -------------------------------------
+ * w[n*n] (host): symmetric conflict weights of n pairs with a zero diagonal.  Restarts r in [r0, r1) of the tabu search
+ * into n_pools balanced pools, each independent of the others: best_cost[r - r0] is the lowest cost the restart
+ * reached, best_step[r - r0] the first step at which it did, assign[(r - r0)*n + a] the pool of pair a at that step
+ * (host arrays).  Limits (MPB_EINVAL): 1 <= n <= 512, 1 <= n_pools <= 32, n_pools <= n, 0 <= r0 <= r1 <= 2^24,
+ * 0 <= iterations <= 2^20 - 1, w symmetric with a zero diagonal. */
+int mpb_pool_search(mpb_ctx* ctx, int32_t n, int32_t n_pools, const uint8_t* w, uint64_t seed, int64_t r0, int64_t r1,
+                    int32_t iterations, int64_t* best_cost, int32_t* best_step, uint8_t* assign);
+
 #ifdef __cplusplus
 }
 #endif

@@ -99,6 +99,8 @@ SIGNATURES = {
     "mpb_dimer_pairs": (C.c_int, [_P, _P, _P, C.c_int64, _P, _P]),
     "mpb_dimer_grid": (C.c_int, [_P, C.c_int32, C.c_int32, C.c_int64, _P, _P, _P, _P, C.POINTER(C.c_int64),
                                   C.POINTER(C.c_int64)]),
+    "mpb_pool_search": (C.c_int, [_P, C.c_int32, C.c_int32, _P, C.c_uint64, C.c_int64, C.c_int64, C.c_int32, _P, _P,
+                                  _P]),
 }
 
 
@@ -343,6 +345,21 @@ class Context:
         if len(pf):
             check(load().mpb_pair_cover3(self.h, ptr(bits), shape[0], shape[2], ptr(pf), ptr(pr), len(pf), ptr(out)))
         return out
+
+    def pool_search(self, w, n_pools: int, seed: int, r0: int, r1: int, iterations: int):
+        """mpb_pool_search: restarts [r0, r1) of the pool search on the symmetric weights w[n, n] -> dict(cost int64[R],
+        step int32[R], assign uint8[R, n]) per restart"""
+        w = np.ascontiguousarray(w, dtype=np.uint8)
+        n = w.shape[0] if w.ndim == 2 else 0
+        nr = max(int(r1) - int(r0), 0)
+        cost = np.zeros(nr, np.int64)
+        step = np.zeros(nr, np.int32)
+        assign = np.zeros((nr, max(n, 1)), np.uint8)
+        if w.ndim != 2 or w.shape[0] != w.shape[1]:
+            raise MpbError(-1, "w must be a square matrix (got shape %s)" % (w.shape,))
+        check(load().mpb_pool_search(self.h, n, n_pools, ptr(w), int(seed) & 0xFFFFFFFFFFFFFFFF, r0, r1, iterations,
+                                     ptr(cost), ptr(step), ptr(assign)))
+        return dict(cost=cost, step=step, assign=assign[:, :n])
 
     def close(self):
         if self.h and not self.is_shared:

@@ -12,7 +12,7 @@ ROOT = os.path.dirname(PKG)
 CSRC = os.path.join(PKG, "csrc")
 LIB = os.path.join(PKG, "libmpb200.so")
 SOURCES = ["mpb200.cu", "mpb_cscan.cu", "mpb_prefilter.cu", "mpb_walk_dev.cu", "mpb_peer.cu", "mpb_dimer.cu", "mpb_walk.cu",
-           "mpb_products.cu"]
+           "mpb_products.cu", "mpb_pools.cu"]
 HEADERS = [os.path.join(CSRC, h) for h in ("mpb_device.cuh", "mpb_host.h", "mpb_cscan.h", "mpb_walk_core.h")] + \
     [os.path.join(ROOT, "include", "mpb200.h")]
 

@@ -71,6 +71,32 @@ def nth_end(sets, e_idx: int, min_end: int = 5, max_end: int = 18) -> str:
     raise IndexError("end index out of range")
 
 
+def grid_hits(ctx, backend, sets_list, threshold: float, comm=None, rows_per_band: int = 0):
+    """finDimer's pair grid over a primer list (base sets per primer): every (i, j >= i) that forms a dimer ->
+    (hits [(i, j, order index, d2)] in (i, j) order on every rank, expansions per primer, pairs tested)"""
+    eng = backend.Dimer(ctx, sets_list, 5, 18, True, loss_table(threshold), dg_consts())
+    n = len(sets_list)
+    rank, world = (comm.rank, comm.world) if comm else (0, 1)
+    band = rows_per_band or max(1, min(n, (1 << 24) // max(1, n) * 8))
+    hits = []
+    tested = 0
+    try:
+        for b, r0 in enumerate(range(0, n, band)):
+            if b % world != rank:              # row bands dealt round-robin to the ranks
+                continue
+            hi, hj, ho, hd, nt = eng.grid(r0, min(n, r0 + band))
+            tested += nt
+            hits.extend(zip(hi.tolist(), hj.tolist(), ho.tolist(), hd.tolist()))
+        n_p = np.diff(eng.off_p)
+    finally:
+        eng.close()
+    if comm and world > 1:                     # hit lists of the ranks: one variable-length gather of int64 quadruples
+        flat, _ = comm.allgather_concat(np.array(hits, np.int64).reshape(-1))
+        hits = sorted(tuple(int(x) for x in h) for h in flat.reshape(-1, 4))
+        tested = int(comm.allreduce_sum(np.array([tested], np.int64))[0])
+    return hits, n_p, tested
+
+
 class Dimer(object):
     """finDimer_V4.py:127-146 constructor arguments"""
 
@@ -102,27 +128,8 @@ class Dimer(object):
         """all dimer rows in (i, j) order"""
         plist = self.primers_list
         sets_list = [sets_of(p.upper()) for p in plist]
-        eng = self._backend.Dimer(self.ctx, sets_list, 5, 18, True, loss_table(self.threshold), dg_consts())
-        n = len(plist)
-        rank, world = (self.comm.rank, self.comm.world) if self.comm else (0, 1)
-        band = rows_per_band or max(1, min(n, (1 << 24) // max(1, n) * 8))
-        hits = []
-        tested = 0
-        try:
-            for b, r0 in enumerate(range(0, n, band)):
-                if b % world != rank:              # row bands dealt round-robin to the ranks
-                    continue
-                hi, hj, ho, hd, nt = eng.grid(r0, min(n, r0 + band))
-                tested += nt
-                hits.extend(zip(hi.tolist(), hj.tolist(), ho.tolist(), hd.tolist()))
-            n_p = np.diff(eng.off_p)
-        finally:
-            eng.close()
-        if self.comm and world > 1:              # hit lists of the ranks: one variable-length gather of int64 quadruples
-            flat, _ = self.comm.allgather_concat(np.array(hits, np.int64).reshape(-1))
-            hits = sorted(tuple(int(x) for x in h) for h in flat.reshape(-1, 4))
-            tested = int(self.comm.allreduce_sum(np.array([tested], np.int64))[0])
-        self.pairs_tested = tested
+        hits, n_p, self.pairs_tested = grid_hits(self.ctx, self._backend, sets_list, self.threshold, self.comm,
+                                                 rows_per_band)
         rows = []
         for i, j, order, d2 in hits:
             end = nth_end(sets_list[i], order // int(n_p[j]))

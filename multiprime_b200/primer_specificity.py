@@ -161,25 +161,25 @@ def run(ref: str, pairs: dict, out: str, v: int = 1, coordinate: str = "1,2,-1",
     return res
 
 
-def argsParse(argv=None):
-    parser = OptionParser('Usage: %prog -r [targets.fa] -i [primers] -f [format] -o [out_prefix]')
+def add_options(parser: OptionParser, out_default: str = "primer_specificity",
+                out_help: str = "<out>.specificity.tsv and <out>.products.tsv"):
+    """the flags -r -i -f -o -v -c -s of this tool; primer_pools takes them too"""
     parser.add_option('-r', '--ref', dest='ref', help='targets: FASTA of unaligned sequences (or a background database).')
     parser.add_option('-i', '--input', dest='input',
                       help='Primer file. One of: final_maxprimers_set.xls, primer.fa, primer_F,primer_R.')
     parser.add_option('-f', '--format', dest='format', help='Format of primer file: xls or fa or seq.')
-    parser.add_option('-o', '--out', dest='out', default="primer_specificity",
-                      help='Output prefix: <out>.specificity.tsv and <out>.products.tsv. default: primer_specificity.')
+    parser.add_option('-o', '--out', dest='out', default=out_default,
+                      help='Output prefix: %s. default: %s.' % (out_help, out_default))
     parser.add_option('-v', '--variation', dest='variation', default=1, type="int",
                       help='Max mismatch number of a primer site. Default: 1.')
     parser.add_option('-c', '--coordinate', dest='coordinate', default="1,2,-1",
                       help='Primer positions where a mismatch disqualifies a site (>0: from the 5\' end, <0: from the 3\' '
                            'end). Default: 1,2,-1.')
     parser.add_option('-s', '--size', dest='size', default="50,2000", help='lo,hi of the product length. Default: 50,2000.')
-    parser.add_option('--max-rows', dest='max_rows', default=MAX_ROWS, type="int",
-                      help='Rows of <out>.products.tsv at most. Default: %d.' % MAX_ROWS)
-    parser.add_option('--device', dest='device', default=0, type="int", help=SUPPRESS_HELP)
-    args = sys.argv[1:] if argv is None else argv
-    (options, rest) = parser.parse_args(args)
+
+
+def check_options(parser: OptionParser, options):
+    """the checks of the flags of add_options (and of --max-rows when the parser has it); options.size -> (lo, hi)"""
     for value, msg in ((options.ref, "Input (targets) file must be specified !!!"),
                        (options.input, "Primer file or sequence must be specified !!!"),
                        (options.format, "Primer file format must be specified !!!")):
@@ -188,7 +188,7 @@ def argsParse(argv=None):
             raise SystemExit("Error: " + msg)
     if options.format not in ("xls", "fa", "seq"):
         raise SystemExit("Error: -f must be xls, fa or seq (got %s)" % options.format)
-    if options.max_rows < 0:
+    if getattr(options, "max_rows", 0) < 0:
         raise SystemExit("Error: --max-rows must be >= 0 (got %d)" % options.max_rows)
     try:
         options.size = tuple(int(x) for x in options.size.split(","))
@@ -197,6 +197,17 @@ def argsParse(argv=None):
     except (ValueError, AssertionError):
         raise SystemExit("Error: -s takes lo,hi and -c a comma-separated list of integers")
     return options
+
+
+def argsParse(argv=None):
+    parser = OptionParser('Usage: %prog -r [targets.fa] -i [primers] -f [format] -o [out_prefix]')
+    add_options(parser)
+    parser.add_option('--max-rows', dest='max_rows', default=MAX_ROWS, type="int",
+                      help='Rows of <out>.products.tsv at most. Default: %d.' % MAX_ROWS)
+    parser.add_option('--device', dest='device', default=0, type="int", help=SUPPRESS_HELP)
+    args = sys.argv[1:] if argv is None else argv
+    (options, rest) = parser.parse_args(args)
+    return check_options(parser, options)
 
 
 def main(argv=None, _backend=None):
