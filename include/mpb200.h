@@ -58,6 +58,8 @@ int mpb_dev_alloc(mpb_ctx* ctx, int64_t bytes, void** out);
 void mpb_dev_free(mpb_ctx* ctx, void* p);
 /* copy between host / device memory on the context's stream; returns after the copy has completed */
 int mpb_ctx_memcpy(mpb_ctx* ctx, void* dst, const void* src, int64_t bytes);
+/* set `bytes` bytes of device memory to `value` on the context's stream; returns after it has completed */
+int mpb_ctx_memset(mpb_ctx* ctx, void* dst, int value, int64_t bytes);
 
 /* Profiling: when enabled every kernel launch is bracketed by CUDA events on the context's stream.
  * mpb_ctx_profile_read sums duration (ms), launch count and algorithmic work units (candidate x sequence
@@ -242,6 +244,32 @@ int mpb_pattern_products(mpb_msa* msa, int32_t n_pat, const uint32_t* allow, con
                          int32_t n_rec, const int64_t* rec_off, const int64_t* rec_len, int32_t lo, int32_t hi,
                          const uint8_t* list, int64_t chunk, int64_t max_rows, int64_t* comb, int64_t* uni, int64_t* rows,
                          int64_t* n_listed, int64_t* stats);
+
+/* Coverage of every pair by its own two patterns (primer_select.py).  Rows, stride, records and allow / lens / strict / v
+ * as in mpb_pattern_products; the n_pat = 4 * pairs patterns are in primer_coverage's Panel order: F, RC(R), R, RC(F)
+ * of pair 0, then of pair 1, ...  An amplicon of pair q is a site of pattern 4q at x and of 4q+1 at y (+ strand), or of
+ * 4q+2 at x and 4q+3 at y (- strand), in one record, with y >= x + L(left) and y + L(right) - x in [lo, hi].  The call
+ * ORs bit r of amp[q*words + r/32] for every record r where pair q has an amplicon, and the same bit of perf[...] when one
+ * of them has no mismatch on either site (amp / perf: device memory the caller zeroes; offset them for a block of
+ * pairs).  max_sites: the search's first capacity (0: 2^24); when the search finds more sites it runs once more with
+ * room for all of them, so a caller that knows the count (from the previous call of a block loop) saves that second
+ * pass.  stats[3]: search hits, left sites, right sites.  Device memory is bounded by the sites of the call; products
+ * are never stored.  Limits (MPB_EINVAL): n_pat a positive multiple of 4, n_rec < 2^31, words >= ceil(n_rec / 32),
+ * 0 < lo <= hi, 0 <= max_sites <= 2^31, every record ending inside the rows (rec_off + rec_len <= rows * stride),
+ * bits(n_pat) + bits(rows * stride) + 4 <= 64 (the site key). */
+int mpb_pattern_cover(mpb_msa* msa, int32_t n_pat, const uint32_t* allow, const int32_t* lens, const uint32_t* strict,
+                      int32_t v, int64_t stride, int32_t n_rec, const int64_t* rec_off, const int64_t* rec_len, int32_t lo,
+                      int32_t hi, int64_t words, uint32_t* amp, uint32_t* perf, int64_t max_sites, int64_t* stats);
+/* The greedy step over a coverage matrix amp / perf [n_rows][words] (device, words a positive multiple of 4, 16-byte
+ * aligned) and the covered vectors covered / covered_perfect [words] (device): for the rows cand[n_cand] (host),
+ * gains[2i] = popcount(amp[cand[i]] & ~covered) and gains[2i+1] = popcount(perf[cand[i]] & ~covered_perfect) (host or
+ * device).  Rows that are not listed are not read. */
+int mpb_cover_gains(mpb_ctx* ctx, const uint32_t* amp, const uint32_t* perf, int64_t n_rows, int64_t words,
+                    const uint32_t* covered, const uint32_t* covered_perfect, const int32_t* cand, int64_t n_cand,
+                    int64_t* gains);
+/* covered |= amp[row], covered_perfect |= perf[row] (the arrays of mpb_cover_gains) */
+int mpb_cover_take(mpb_ctx* ctx, const uint32_t* amp, const uint32_t* perf, int64_t n_rows, int64_t words, int64_t row,
+                   uint32_t* covered, uint32_t* covered_perfect);
 
 /* Per (window, sequence) haplotype key, for the JSON side files (core:1172-1176): the table key of the
  * sequence's k-mer, MPB_KEY_IUPAC for rows whose window holds IUPAC cells. out[nw*n_seq]. */

@@ -28,6 +28,7 @@ SIGNATURES = {
     "mpb_ctx_sync": (C.c_int, [_P]),
     "mpb_ctx_launches": (C.c_int64, [_P]),
     "mpb_ctx_memcpy": (C.c_int, [_P, _P, _P, C.c_int64]),
+    "mpb_ctx_memset": (C.c_int, [_P, _P, C.c_int, C.c_int64]),
     "mpb_dev_alloc": (C.c_int, [_P, C.c_int64, C.POINTER(_P)]),
     "mpb_dev_free": (None, [_P, _P]),
     "mpb_ctx_profile": (C.c_int, [_P, C.c_int]),
@@ -101,6 +102,10 @@ SIGNATURES = {
                                   C.POINTER(C.c_int64)]),
     "mpb_pool_search": (C.c_int, [_P, C.c_int32, C.c_int32, _P, C.c_uint64, C.c_int64, C.c_int64, C.c_int32, _P, _P,
                                   _P]),
+    "mpb_pattern_cover": (C.c_int, [_P, C.c_int32, _P, _P, _P, C.c_int32, C.c_int64, C.c_int32, _P, _P, C.c_int32,
+                                    C.c_int32, C.c_int64, _P, _P, C.c_int64, _P]),
+    "mpb_cover_gains": (C.c_int, [_P, _P, _P, C.c_int64, C.c_int64, _P, _P, _P, C.c_int64, _P]),
+    "mpb_cover_take": (C.c_int, [_P, _P, _P, C.c_int64, C.c_int64, C.c_int64, _P, _P]),
 }
 
 
@@ -245,6 +250,9 @@ class DevBuf:
         check(load().mpb_ctx_memcpy(self.ctx.h, ptr(out), C.c_void_p(self.p), self.nbytes))
         return out
 
+    def zero(self):
+        check(load().mpb_ctx_memset(self.ctx.h, C.c_void_p(self.p), 0, self.nbytes))
+
     def close(self):
         if self.p and self.ctx.h:
             load().mpb_dev_free(self.ctx.h, C.c_void_p(self.p))
@@ -255,6 +263,43 @@ class DevBuf:
             self.close()
         except Exception:
             pass
+
+
+class CoverMatrix:
+    """mpb_pattern_cover's bits in HBM: amp / perf [n_rows, words] (bit r of row c set when pair c amplifies record r /
+    has a perfect amplicon there) and the covered / covered_perfect vectors of a greedy over them, all zeroed at the
+    start.  words = ceil(n_rec / 128) * 4 (at least 4): rows are whole 128-bit loads."""
+
+    def __init__(self, ctx: "Context", n_rows: int, n_rec: int):
+        self.ctx, self.n_rows, self.n_rec = ctx, int(n_rows), int(n_rec)
+        self.words = words_of(n_rec)
+        self.buf = DevBuf(ctx, (2 * self.n_rows + 2, self.words), np.uint32)     # amp rows, perf rows, the two vectors
+        try:
+            self.buf.zero()
+        except MpbError:
+            self.buf.close()
+            raise
+        self.amp, self.perf = self.buf.at(0), self.buf.at(self.n_rows)
+        self.covered, self.covered_perfect = self.buf.at(2 * self.n_rows), self.buf.at(2 * self.n_rows + 1)
+
+    def to_host(self):
+        """(amp, perf, covered, covered_perfect) as uint32 arrays"""
+        a = self.buf.to_host()
+        n = self.n_rows
+        return a[:n], a[n:2 * n], a[2 * n], a[2 * n + 1]
+
+    def close(self):
+        self.buf.close()
+
+
+def words_of(n_rec: int) -> int:
+    """32-bit words of one CoverMatrix row"""
+    return max(4, -(-int(n_rec) // 128) * 4)
+
+
+def cover_bytes(n_rows: int, n_rec: int) -> int:
+    """device bytes of a CoverMatrix"""
+    return (2 * int(n_rows) + 2) * words_of(n_rec) * 4
 
 
 class Context:
@@ -360,6 +405,20 @@ class Context:
         check(load().mpb_pool_search(self.h, n, n_pools, ptr(w), int(seed) & 0xFFFFFFFFFFFFFFFF, r0, r1, iterations,
                                      ptr(cost), ptr(step), ptr(assign)))
         return dict(cost=cost, step=step, assign=assign[:, :n])
+
+    def cover_gains(self, mat: CoverMatrix, cand) -> np.ndarray:
+        """mpb_cover_gains -> int64[len(cand), 2]: new targets and new perfect targets of the listed rows"""
+        cand = np.ascontiguousarray(cand, dtype=np.int32)
+        out = np.zeros((len(cand), 2), np.int64)
+        check(load().mpb_cover_gains(self.h, C.c_void_p(mat.amp), C.c_void_p(mat.perf), mat.n_rows, mat.words,
+                                     C.c_void_p(mat.covered), C.c_void_p(mat.covered_perfect), ptr(cand), len(cand),
+                                     ptr(out)))
+        return out
+
+    def cover_take(self, mat: CoverMatrix, row: int):
+        """mpb_cover_take: the covered vectors |= row `row`"""
+        check(load().mpb_cover_take(self.h, C.c_void_p(mat.amp), C.c_void_p(mat.perf), mat.n_rows, mat.words, int(row),
+                                    C.c_void_p(mat.covered), C.c_void_p(mat.covered_perfect)))
 
     def close(self):
         if self.h and not self.is_shared:
@@ -502,6 +561,26 @@ class Msa:
                                           hi, ptr(listed), chunk, max_rows, ptr(comb), ptr(uni), ptr(rows), C.byref(n),
                                           ptr(stats)))
         return dict(comb=comb, union=uni, rows=rows[:min(n.value, max_rows)], n_listed=n.value, stats=stats)
+
+    def pattern_cover(self, allow, lens, strict, v: int, stride: int, rec_off, rec_len, lo: int, hi: int,
+                      mat: CoverMatrix, row0: int = 0, max_sites: int = 0) -> np.ndarray:
+        """mpb_pattern_cover: the amp / perf bits of the pairs row0, row0 + 1, ... of mat (four patterns each, Panel
+        order) over the records -> stats int64[3] (search hits, left sites, right sites).  max_sites: the search's
+        first capacity (0: the library's default); a search that finds more sites runs a second time."""
+        allow = np.ascontiguousarray(allow, dtype=np.uint32).reshape(-1, 4)
+        lens = np.ascontiguousarray(lens, dtype=np.int32)
+        strict = np.ascontiguousarray(strict, dtype=np.uint32)
+        rec_off = np.ascontiguousarray(rec_off, dtype=np.int64)
+        rec_len = np.ascontiguousarray(rec_len, dtype=np.int64)
+        if len(rec_off) != mat.n_rec or not 0 <= row0 <= row0 + len(lens) // 4 <= mat.n_rows:
+            raise MpbError(-1, "pairs %d.. / %d records do not fit the %d x %d matrix" % (row0, len(rec_off), mat.n_rows,
+                                                                                          mat.n_rec))
+        stats = np.zeros(3, np.int64)
+        off = row0 * mat.words * 4
+        check(load().mpb_pattern_cover(self.h, len(lens), ptr(allow), ptr(lens), ptr(strict), v, stride, len(rec_off),
+                                       ptr(rec_off), ptr(rec_len), lo, hi, mat.words, C.c_void_p(mat.amp + off),
+                                       C.c_void_p(mat.perf + off), int(max_sites), ptr(stats)))
+        return stats
 
     def seqkeys(self, k: int, win_pos) -> np.ndarray:
         win_pos = np.ascontiguousarray(win_pos, dtype=np.int32)

@@ -137,6 +137,15 @@ extern "C" int mpb_ctx_memcpy(mpb_ctx* ctx, void* dst, const void* src, int64_t 
     return 0;
 }
 
+extern "C" int mpb_ctx_memset(mpb_ctx* ctx, void* dst, int value, int64_t bytes) {
+    if (!ctx || !dst || bytes < 0) return fail(MPB_EINVAL, "bad argument");
+    if (!mpb_is_device_ptr(dst)) return fail(MPB_EINVAL, "dst must be device memory");
+    CK(cudaSetDevice(ctx->device));
+    CK(cudaMemsetAsync(dst, value, (size_t)bytes, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    return 0;
+}
+
 extern "C" int mpb_ctx_profile(mpb_ctx* ctx, int enable) {
     if (!ctx) return fail(MPB_EINVAL, "ctx is NULL");
     ctx->profile = enable != 0;

@@ -550,3 +550,247 @@ extern "C" int mpb_pattern_products(mpb_msa* m, int32_t n_pat, const uint32_t* a
     uni[1] = (int64_t)u[1];
     return 0;
 }
+
+
+// ---- mpb_pattern_cover / mpb_cover_gains / mpb_cover_take (primer_select.py) ---------------------------------------
+// Each pair's own amplicons only, as one bit per (pair, record) that stays in HBM:
+//   search   k_pattern_sites into device buffers, as above;
+//   filter   k_cover_filter: the sites k_products_filter keeps, each packed into one 64-bit key
+//              pattern << (pos_bits + 4) | stream position << 4 | mismatches
+//            so one sort puts every pattern's sites in stream order, the runs of 4q .. 4q+3 one after the other;
+//   sort     cub::DeviceRadixSort of the keys;
+//   join     k_cover_join: a thread per left site (pattern 4q: F, 4q+2: R) binary-searches the run of its right pattern
+//            (4q+1: RC(R), 4q+3: RC(F)) for the first site in the product window; any site there is an amplicon, so it
+//            sets the record's bit of pair q, and the perfect bit when the left site and some right site in the window
+//            have no mismatch.  Only sites and bits are stored, never products.
+#define COVER_MAX_REC ((1ll << 31) - 1)
+
+__global__ void k_cover_filter(const int32_t* __restrict__ hp, const int32_t* __restrict__ hr, const int32_t* __restrict__ hx,
+                               const int32_t* __restrict__ hm, long long n, const int32_t* __restrict__ pat_len,
+                               long long stride, const int64_t* __restrict__ off, const int64_t* __restrict__ len,
+                               int n_rec, int pos_bits, unsigned long long* __restrict__ key,
+                               unsigned long long* __restrict__ n_key) {
+    for (long long k = (long long)blockIdx.x * blockDim.x + threadIdx.x; k < n; k += (long long)gridDim.x * blockDim.x) {
+        const long long x = hx[k];
+        if (x >= stride) continue;
+        const long long g = (long long)hr[k] * stride + x;
+        const int r = find_record(off, n_rec, g);
+        if (r < 0) continue;
+        const int p = hp[k];
+        if (g + __ldg(pat_len + p) > __ldg(off + r) + __ldg(len + r)) continue;
+        const unsigned long long slot = atomicAdd(n_key, 1ull);
+        key[slot] = (unsigned long long)p << (pos_bits + 4) | (unsigned long long)g << 4 | (unsigned long long)hm[k];
+        if ((p & 1) == 0) atomicAdd(n_key + 1, 1ull);  // left sites
+    }
+}
+
+__global__ void k_cover_join(const unsigned long long* __restrict__ key, long long n, int pos_bits,
+                             const int32_t* __restrict__ pat_len, int lo, int hi, const int64_t* __restrict__ off,
+                             const int64_t* __restrict__ len, int n_rec, long long words, uint32_t* __restrict__ amp,
+                             uint32_t* __restrict__ perf) {
+    const unsigned long long pos_mask = (1ull << pos_bits) - 1;
+    for (long long k = (long long)blockIdx.x * blockDim.x + threadIdx.x; k < n; k += (long long)gridDim.x * blockDim.x) {
+        const unsigned long long kk = key[k];
+        const int p = (int)(kk >> (pos_bits + 4));
+        if (p & 1) continue;  // right sites are what the left sites look for
+        const long long g = (long long)((kk >> 4) & pos_mask);
+        const int lm = (int)(kk & 15);
+        const int r = find_record(off, n_rec, g);
+        const long long end = __ldg(off + r) + __ldg(len + r);
+        const int ll = __ldg(pat_len + p), rl = __ldg(pat_len + p + 1);
+        const long long ylo = g + max(ll, lo - rl), yhi = min(g + (long long)hi - rl, end - rl);
+        if (ylo > yhi) continue;
+        const unsigned long long base = (unsigned long long)(p + 1) << (pos_bits + 4);
+        const unsigned long long want = base | (unsigned long long)ylo << 4, last = base | (unsigned long long)yhi << 4 | 15;
+        long long q0 = k + 1, q1 = n;  // the right run follows the left one
+        while (q0 < q1) {
+            const long long mid = (q0 + q1) >> 1;
+            if (__ldg(key + mid) < want) q0 = mid + 1;
+            else q1 = mid;
+        }
+        if (q0 >= n || __ldg(key + q0) > last) continue;
+        const long long word = (long long)(p >> 2) * words + (r >> 5);
+        const uint32_t bit = 1u << (r & 31);
+        if (!(__ldcg(amp + word) & bit)) atomicOr(amp + word, bit);
+        if (lm != 0 || (__ldcg(perf + word) & bit)) continue;
+        for (long long q = q0; q < n; ++q) {  // stop at the first perfect product
+            const unsigned long long rk = __ldg(key + q);
+            if (rk > last) break;
+            if ((rk & 15) == 0) {
+                atomicOr(perf + word, bit);
+                break;
+            }
+        }
+    }
+}
+
+extern "C" int mpb_pattern_cover(mpb_msa* m, int32_t n_pat, const uint32_t* allow, const int32_t* lens,
+                                 const uint32_t* strict, int32_t v, int64_t stride, int32_t n_rec, const int64_t* rec_off,
+                                 const int64_t* rec_len, int32_t lo, int32_t hi, int64_t words, uint32_t* amp,
+                                 uint32_t* perf, int64_t max_sites, int64_t* stats) {
+    if (!m || !allow || !lens || !strict || !amp || !perf || !stats || (n_rec > 0 && (!rec_off || !rec_len)))
+        return fail(MPB_EINVAL, "NULL argument");
+    if (v < 0) return fail(MPB_EINVAL, "negative mismatch bound %d", v);
+    if (n_pat < 4 || n_pat % 4) return fail(MPB_EINVAL, "%d patterns: four per pair are needed", n_pat);
+    if (n_rec < 0 || (long long)n_rec > COVER_MAX_REC) return fail(MPB_EINVAL, "bad n_rec %d", n_rec);
+    if (words < (n_rec + 31) / 32) return fail(MPB_EINVAL, "%lld words hold fewer than %d records", (long long)words, n_rec);
+    if (lo < 1 || lo > hi) return fail(MPB_EINVAL, "product lengths %d..%d: need 0 < lo <= hi", lo, hi);
+    if (max_sites < 0 || max_sites > (1ll << 31)) return fail(MPB_EINVAL, "max_sites %lld outside 0..2^31", (long long)max_sites);
+    if (!mpb_is_device_ptr(amp) || !mpb_is_device_ptr(perf)) return fail(MPB_EINVAL, "amp and perf must be device memory");
+    if (stride < 1 || stride > (1ll << 60) / (m->n_seq > 0 ? m->n_seq : 1))
+        return fail(MPB_EINVAL, "%lld rows of stride %lld: the site key needs more than 64 bits", (long long)m->n_seq,
+                    (long long)stride);
+    const int pat_bits = bits_for(n_pat), pos_bits = bits_for(m->n_seq * stride);
+    if (pat_bits + pos_bits + 4 > 64)
+        return fail(MPB_EINVAL, "%d patterns over %lld rows of stride %lld: the site key needs %d + %d + 4 > 64 bits", n_pat,
+                    (long long)m->n_seq, (long long)stride, pat_bits, pos_bits);
+    for (int r = 0; r < n_rec; ++r)
+        if (rec_len[r] < 0 || rec_off[r] < 0 || (r > 0 && rec_off[r] < rec_off[r - 1] + rec_len[r - 1]))
+            return fail(MPB_EINVAL, "record %d: offset %lld / length %lld overlap the record before it", r,
+                        (long long)rec_off[r], (long long)rec_len[r]);
+    if (n_rec > 0 && rec_off[n_rec - 1] + rec_len[n_rec - 1] > m->n_seq * stride)  // keys and windows stay in pos_bits
+        return fail(MPB_EINVAL, "record %d ends at %lld, past the %lld stream columns of the rows", n_rec - 1,
+                    (long long)(rec_off[n_rec - 1] + rec_len[n_rec - 1]), (long long)(m->n_seq * stride));
+    mpb_ctx* ctx = m->ctx;
+    CK(cudaSetDevice(ctx->device));
+    for (int s = 0; s < 3; ++s) stats[s] = 0;
+    if (n_rec == 0) return 0;
+
+    // the search runs once when the caller's capacity holds its sites, twice otherwise (counted, then stored)
+    DMem hp, hr, hx, hm;
+    int64_t cap = max_sites > 0 ? max_sites : 1 << 24, n_hits = 0;
+    for (;;) {
+        CK(hp.reserve(cap * 4));
+        CK(hr.reserve(cap * 4));
+        CK(hx.reserve(cap * 4));
+        CK(hm.reserve(cap * 4));
+        const int rc = mpb_pattern_search(m, n_pat, allow, lens, strict, v, cap, hp.as<int32_t>(), hr.as<int32_t>(),
+                                          hx.as<int32_t>(), hm.as<int32_t>(), &n_hits);
+        if (rc) return rc;
+        if (n_hits <= cap) break;
+        cap = n_hits + 16;
+    }
+    stats[0] = n_hits;
+
+    DMem d_pl, d_off, d_len, d_cnt, k1, k2, tmp;
+    CK(d_pl.reserve(n_pat * 4));
+    CK(d_off.reserve(n_rec * 8));
+    CK(d_len.reserve(n_rec * 8));
+    CK(d_cnt.reserve(16));
+    CK(cudaMemcpyAsync(d_pl.p, lens, n_pat * 4, cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemcpyAsync(d_off.p, rec_off, n_rec * 8, cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemcpyAsync(d_len.p, rec_len, n_rec * 8, cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemsetAsync(d_cnt.p, 0, 16, ctx->stream));
+    const long long nh = n_hits > 0 ? n_hits : 1;
+    CK(k1.reserve(nh * 8));
+    CK(k2.reserve(nh * 8));
+    unsigned long long* cnt = d_cnt.as<unsigned long long>();
+    if (n_hits > 0)
+        MPB_LAUNCH_NAMED(ctx, "k_cover_filter", k_cover_filter, grid_of(n_hits), 256, 0, hp.as<int32_t>(), hr.as<int32_t>(),
+                         hx.as<int32_t>(), hm.as<int32_t>(), (long long)n_hits, d_pl.as<int32_t>(), (long long)stride,
+                         d_off.as<int64_t>(), d_len.as<int64_t>(), (int)n_rec, pos_bits, k1.as<unsigned long long>(), cnt);
+    unsigned long long nk[2];
+    CK(cudaMemcpyAsync(nk, cnt, 16, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    hp.release(), hr.release(), hx.release(), hm.release();
+    const long long n_key = (long long)nk[0];
+    stats[1] = (int64_t)nk[1];
+    stats[2] = n_key - (int64_t)nk[1];
+    if (stats[1] == 0 || stats[2] == 0) return 0;
+    {
+        unsigned long long *a = k1.as<unsigned long long>(), *b = k2.as<unsigned long long>();
+        const int rc = cub_run(ctx, "k_cover_sort", tmp, [&](void* t, size_t& bytes) {
+            return cub::DeviceRadixSort::SortKeys(t, bytes, a, b, n_key, 0, pat_bits + pos_bits + 4, ctx->stream);
+        });
+        if (rc) return rc;
+    }
+    k1.release();
+    MPB_LAUNCH_NAMED(ctx, "k_cover_join", k_cover_join, grid_of(n_key), 256, 0, k2.as<unsigned long long>(), n_key,
+                     pos_bits, d_pl.as<int32_t>(), (int)lo, (int)hi, d_off.as<int64_t>(), d_len.as<int64_t>(), (int)n_rec,
+                     (long long)words, amp, perf);
+    CK(cudaStreamSynchronize(ctx->stream));
+    return 0;
+}
+
+// gains[2i] = popcount(amp[cand[i]] & ~covered), gains[2i+1] = popcount(perf[cand[i]] & ~covered_perfect): one warp per
+// listed row, 128-bit loads, a warp-shuffle sum and one store per row; rows that are not listed are never read
+#define GAINS_WARPS 8
+__global__ void __launch_bounds__(GAINS_WARPS * 32)
+k_cover_gains(const uint4* __restrict__ amp, const uint4* __restrict__ perf, long long words4,
+              const uint4* __restrict__ cov, const uint4* __restrict__ covp, const int32_t* __restrict__ cand, long long n,
+              int64_t* __restrict__ gains) {
+    const long long i = (long long)blockIdx.x * GAINS_WARPS + (threadIdx.x >> 5);
+    const int lane = threadIdx.x & 31;
+    if (i >= n) return;
+    const long long row = (long long)__ldg(cand + i) * words4;
+    unsigned a = 0, b = 0;
+    for (long long w = lane; w < words4; w += 32) {
+        const uint4 x = __ldg(amp + row + w), y = __ldg(perf + row + w), c = __ldg(cov + w), d = __ldg(covp + w);
+        a += __popc(x.x & ~c.x) + __popc(x.y & ~c.y) + __popc(x.z & ~c.z) + __popc(x.w & ~c.w);
+        b += __popc(y.x & ~d.x) + __popc(y.y & ~d.y) + __popc(y.z & ~d.z) + __popc(y.w & ~d.w);
+    }
+#pragma unroll
+    for (int s = 16; s > 0; s >>= 1) {
+        a += __shfl_xor_sync(0xFFFFFFFFu, a, s);
+        b += __shfl_xor_sync(0xFFFFFFFFu, b, s);
+    }
+    if (lane == 0) {
+        gains[2 * i] = a;
+        gains[2 * i + 1] = b;
+    }
+}
+
+__global__ void k_cover_take(const uint32_t* __restrict__ amp, const uint32_t* __restrict__ perf, long long words,
+                             uint32_t* __restrict__ cov, uint32_t* __restrict__ covp) {
+    for (long long w = (long long)blockIdx.x * blockDim.x + threadIdx.x; w < words; w += (long long)gridDim.x * blockDim.x) {
+        cov[w] |= amp[w];
+        covp[w] |= perf[w];
+    }
+}
+
+static int cover_args(const uint32_t* amp, const uint32_t* perf, int64_t n_rows, int64_t words, const uint32_t* cov,
+                      const uint32_t* covp) {
+    if (!amp || !perf || !cov || !covp) return fail(MPB_EINVAL, "NULL argument");
+    if (n_rows < 0 || words < 4 || words % 4)
+        return fail(MPB_EINVAL, "%lld rows of %lld words: need rows >= 0 and words a positive multiple of 4",
+                    (long long)n_rows, (long long)words);
+    for (const void* p : {(const void*)amp, (const void*)perf, (const void*)cov, (const void*)covp})
+        if (((uintptr_t)p & 15) || !mpb_is_device_ptr(p))
+            return fail(MPB_EINVAL, "amp, perf and the covered vectors must be 16-byte aligned device memory");
+    return 0;
+}
+
+extern "C" int mpb_cover_gains(mpb_ctx* ctx, const uint32_t* amp, const uint32_t* perf, int64_t n_rows, int64_t words,
+                               const uint32_t* covered, const uint32_t* covered_perfect, const int32_t* cand,
+                               int64_t n_cand, int64_t* gains) {
+    if (!ctx || (n_cand > 0 && (!cand || !gains))) return fail(MPB_EINVAL, "NULL argument");
+    if (int rc = cover_args(amp, perf, n_rows, words, covered, covered_perfect)) return rc;
+    if (n_cand < 0 || n_cand > (1ll << 31) - 1) return fail(MPB_EINVAL, "bad n_cand %lld", (long long)n_cand);
+    for (int64_t i = 0; i < n_cand; ++i)
+        if (cand[i] < 0 || cand[i] >= n_rows)
+            return fail(MPB_EINVAL, "candidate %lld: row %d outside 0..%lld", (long long)i, cand[i], (long long)n_rows - 1);
+    if (n_cand == 0) return 0;
+    CK(cudaSetDevice(ctx->device));
+    InBuf ic(ctx, cand, (size_t)n_cand * 4);
+    OutBuf og(ctx, gains, (size_t)n_cand * 16);
+    if (ic.rc || og.rc) return MPB_ECUDA;
+    ctx->pending_units = (double)n_cand * (double)words * 8.0;  // bytes of the listed rows
+    MPB_LAUNCH(ctx, k_cover_gains, (unsigned)((n_cand + GAINS_WARPS - 1) / GAINS_WARPS), GAINS_WARPS * 32, 0,
+               (const uint4*)amp, (const uint4*)perf, (long long)(words / 4), (const uint4*)covered,
+               (const uint4*)covered_perfect, ic.dev<int32_t>(), (long long)n_cand, og.dev<int64_t>());
+    CK(og.finish());
+    CK(cudaStreamSynchronize(ctx->stream));
+    return 0;
+}
+
+extern "C" int mpb_cover_take(mpb_ctx* ctx, const uint32_t* amp, const uint32_t* perf, int64_t n_rows, int64_t words,
+                              int64_t row, uint32_t* covered, uint32_t* covered_perfect) {
+    if (!ctx) return fail(MPB_EINVAL, "NULL argument");
+    if (int rc = cover_args(amp, perf, n_rows, words, covered, covered_perfect)) return rc;
+    if (row < 0 || row >= n_rows) return fail(MPB_EINVAL, "row %lld outside 0..%lld", (long long)row, (long long)n_rows - 1);
+    CK(cudaSetDevice(ctx->device));
+    MPB_LAUNCH(ctx, k_cover_take, grid_of(words), 256, 0, amp + row * words, perf + row * words, (long long)words, covered,
+               covered_perfect);
+    CK(cudaStreamSynchronize(ctx->stream));
+    return 0;
+}

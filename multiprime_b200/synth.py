@@ -159,3 +159,32 @@ def write_pcr_targets(path: str, n_targets: int = 65536, length: int = 10_000, n
                 out.append(b">t%07d\n" % (c0 + i) + letters[s].tobytes() + b"\n")
             fh.write(b"".join(out))
     return pairs
+
+
+def pcr_candidate_pool(n_pairs: int = 2048, length: int = 10_000, seed: int = 20241015):
+    """A candidate pool for the targets of write_pcr_targets (tools/bench_select.py): the generator's first draws (root,
+    clade columns, clade shifts) are replayed, and 20-mer pairs (products of 220..1320 bases) are cut in turn from the
+    root and from its 8 clade variants.  Most forward primers end on a clade column, whose base is then a strict 3'
+    mismatch on the targets of some clades, so no single pair amplifies every target.  write_pcr_targets' output does
+    not depend on this function.  Returns {name: (F, R)}."""
+    rng = np.random.Generator(np.random.PCG64([seed, 0x9C2]))
+    root = rng.integers(0, 4, length).astype(np.uint8)
+    clade_cols = rng.choice(length, (8, 40))
+    clade_shift = rng.integers(1, 4, (8, 40)).astype(np.uint8)
+    variants = [root]
+    for k in range(8):
+        x = root.copy()
+        x[clade_cols[k]] = (x[clade_cols[k]] + clade_shift[k]) % 4
+        variants.append(x)
+    pick = np.random.Generator(np.random.PCG64([seed, 0x5E1]))
+    pairs = {}
+    for q in range(n_pairs):
+        src = variants[q % 9]
+        a = int(clade_cols[int(pick.integers(0, 8)), int(pick.integers(0, 40))]) - 19
+        if not 250 <= a <= length - 1600 or pick.random() < 0.2:
+            a = int(pick.integers(250, length - 1600))
+        b = a + int(pick.integers(200, 1300))
+        f = "".join("ACGT"[x] for x in src[a:a + 20])
+        r = "".join("ACGT"[3 - x] for x in src[b:b + 20][::-1])
+        pairs["cand%04d_v%d" % (q, q % 9)] = (f, r)
+    return pairs
