@@ -271,6 +271,36 @@ int mpb_cover_gains(mpb_ctx* ctx, const uint32_t* amp, const uint32_t* perf, int
 int mpb_cover_take(mpb_ctx* ctx, const uint32_t* amp, const uint32_t* perf, int64_t n_rows, int64_t words, int64_t row,
                    uint32_t* covered, uint32_t* covered_perfect);
 
+/* A resident site list: the filtered sites of every pattern of a panel (n_pat = 4 * pairs, Panel order, lens[n_pat]
+ * host) over one set of records (rec_off / rec_len [n_rec] host, as in mpb_pattern_cover) in a stream of n_pos columns,
+ * kept in device memory for the joins of primer_select.py --cross / --background.  One 64-bit key per site:
+ * stream position << (bits(n_pat) + 4) | pattern << 4 | mismatches.  Limits (MPB_EINVAL): bits(n_pat) + bits(n_pos) + 4
+ * <= 64, every record ending inside n_pos. */
+typedef struct mpb_site_list mpb_site_list;
+int mpb_site_list_create(mpb_ctx* ctx, int32_t n_pat, const int32_t* lens, int64_t n_pos, int32_t n_rec,
+                         const int64_t* rec_off, const int64_t* rec_len, mpb_site_list** out);
+void mpb_site_list_destroy(mpb_site_list* list);
+/* mpb_pattern_cover on the patterns pat0 .. pat0 + n_pat - 1 of the list (pat0 a multiple of 4; lens and records equal
+ * to the list's), with its filtered sites also appended to the list: the same single search.  amp = perf = NULL only
+ * searches and keeps (no sort, no join; words is not read).  A list that cannot grow fails with MPB_ENOMEM and a message
+ * that names the bytes. */
+int mpb_pattern_cover_keep(mpb_msa* msa, int32_t n_pat, const uint32_t* allow, const int32_t* lens, const uint32_t* strict,
+                           int32_t v, int64_t stride, int32_t n_rec, const int64_t* rec_off, const int64_t* rec_len,
+                           int32_t lo, int32_t hi, int64_t words, uint32_t* amp, uint32_t* perf, int64_t max_sites,
+                           int64_t* stats, mpb_site_list* list, int32_t pat0);
+/* Sort every kept key once (stream order; a sealed list takes no more sites): *n_sites = the list's sites. */
+int mpb_site_list_seal(mpb_site_list* list, int64_t* n_sites);
+/* The first min(cap, sites) keys in list order into keys[] (host); *n_sites = the list's sites. */
+int mpb_site_list_keys(mpb_site_list* list, int64_t cap, uint64_t* keys, int64_t* n_sites);
+/* The products between the taken pair `pair` (t) and every pair c whose bit c of eligible[ceil(pairs / 32)] (host) is set,
+ * on a sealed list: a left site of primer i at x and a right site of primer j at y in one record, with y >= x + L_i and
+ * y + L_j - x in [lo, hi], i of one pair and j of the other.  bits[pairs] (host): bit side << 2 | primer of c << 1 |
+ * primer of t of byte c (side 0: t's primer is the left one; primer 0 = F, 1 = R). */
+int mpb_sites_cross(mpb_site_list* list, int32_t lo, int32_t hi, int32_t pair, const uint32_t* eligible, uint8_t* bits);
+/* Each pair's products of its own primers on a sealed list: bits[pairs] (host), bit left primer << 1 | right primer of
+ * byte q set when pair q's (F, F), (F, R), (R, F) or (R, R) has a product. */
+int mpb_sites_own(mpb_site_list* list, int32_t lo, int32_t hi, uint8_t* bits);
+
 /* Per (window, sequence) haplotype key, for the JSON side files (core:1172-1176): the table key of the
  * sequence's k-mer, MPB_KEY_IUPAC for rows whose window holds IUPAC cells. out[nw*n_seq]. */
 #define MPB_KEY_IUPAC 0xFFFFFFFFFFFFFFFEull

@@ -106,6 +106,14 @@ SIGNATURES = {
                                     C.c_int32, C.c_int64, _P, _P, C.c_int64, _P]),
     "mpb_cover_gains": (C.c_int, [_P, _P, _P, C.c_int64, C.c_int64, _P, _P, _P, C.c_int64, _P]),
     "mpb_cover_take": (C.c_int, [_P, _P, _P, C.c_int64, C.c_int64, C.c_int64, _P, _P]),
+    "mpb_site_list_create": (C.c_int, [_P, C.c_int32, _P, C.c_int64, C.c_int32, _P, _P, C.POINTER(_P)]),
+    "mpb_site_list_destroy": (None, [_P]),
+    "mpb_pattern_cover_keep": (C.c_int, [_P, C.c_int32, _P, _P, _P, C.c_int32, C.c_int64, C.c_int32, _P, _P, C.c_int32,
+                                         C.c_int32, C.c_int64, _P, _P, C.c_int64, _P, _P, C.c_int32]),
+    "mpb_site_list_seal": (C.c_int, [_P, C.POINTER(C.c_int64)]),
+    "mpb_site_list_keys": (C.c_int, [_P, C.c_int64, _P, C.POINTER(C.c_int64)]),
+    "mpb_sites_cross": (C.c_int, [_P, C.c_int32, C.c_int32, C.c_int32, _P, _P]),
+    "mpb_sites_own": (C.c_int, [_P, C.c_int32, C.c_int32, _P]),
 }
 
 
@@ -290,6 +298,57 @@ class CoverMatrix:
 
     def close(self):
         self.buf.close()
+
+
+class SiteList:
+    """mpb_site_list: the filtered sites of a panel's n_pat patterns (lens[n_pat]) over the records rec_off / rec_len of
+    a stream of n_pos columns, kept in HBM by Msa.pattern_cover_keep, sealed once, then joined (cross / own)"""
+
+    def __init__(self, ctx: "Context", lens, n_pos: int, rec_off, rec_len):
+        self.ctx = ctx
+        lens = np.ascontiguousarray(lens, dtype=np.int32)
+        rec_off = np.ascontiguousarray(rec_off, dtype=np.int64)
+        rec_len = np.ascontiguousarray(rec_len, dtype=np.int64)
+        self.n_pairs = len(lens) // 4
+        h = C.c_void_p()
+        check(load().mpb_site_list_create(ctx.h, len(lens), ptr(lens), int(n_pos), len(rec_off), ptr(rec_off),
+                                          ptr(rec_len), C.byref(h)))
+        self.h = h
+
+    def seal(self) -> int:
+        """sort the kept sites into stream order -> their number"""
+        n = C.c_int64()
+        check(load().mpb_site_list_seal(self.h, C.byref(n)))
+        return n.value
+
+    def keys(self) -> np.ndarray:
+        """the list's keys (position << (bits(n_pat) + 4) | pattern << 4 | mismatches) in list order"""
+        n = C.c_int64()
+        check(load().mpb_site_list_keys(self.h, 0, None, C.byref(n)))
+        out = np.zeros(n.value, np.uint64)
+        check(load().mpb_site_list_keys(self.h, len(out), ptr(out), C.byref(n)))
+        return out
+
+    def cross(self, lo: int, hi: int, pair: int, eligible) -> np.ndarray:
+        """mpb_sites_cross -> uint8[pairs]: the products between pair `pair` and the pairs flagged in eligible
+        (bool[pairs]), bit side << 2 | primer of the pair << 1 | primer of `pair`"""
+        el = np.packbits(np.asarray(eligible, bool), bitorder="little")
+        el = np.ascontiguousarray(np.pad(el, (0, -len(el) % 4)).view(np.uint32))
+        out = np.zeros(self.n_pairs, np.uint8)
+        check(load().mpb_sites_cross(self.h, lo, hi, int(pair), ptr(el), ptr(out)))
+        return out
+
+    def own(self, lo: int, hi: int) -> np.ndarray:
+        """mpb_sites_own -> uint8[pairs]: bit left primer << 1 | right primer when the pair's own two primers form
+        that product"""
+        out = np.zeros(self.n_pairs, np.uint8)
+        check(load().mpb_sites_own(self.h, lo, hi, ptr(out)))
+        return out
+
+    def close(self):
+        if self.h:
+            load().mpb_site_list_destroy(self.h)
+            self.h = None
 
 
 def words_of(n_rec: int) -> int:
@@ -580,6 +639,29 @@ class Msa:
         check(load().mpb_pattern_cover(self.h, len(lens), ptr(allow), ptr(lens), ptr(strict), v, stride, len(rec_off),
                                        ptr(rec_off), ptr(rec_len), lo, hi, mat.words, C.c_void_p(mat.amp + off),
                                        C.c_void_p(mat.perf + off), int(max_sites), ptr(stats)))
+        return stats
+
+    def pattern_cover_keep(self, allow, lens, strict, v: int, stride: int, rec_off, rec_len, lo: int, hi: int,
+                           mat: CoverMatrix | None, row0: int, max_sites: int, sites: "SiteList") -> np.ndarray:
+        """mpb_pattern_cover_keep: pattern_cover (mat None: no matrix, search only) that also appends its filtered
+        sites to `sites` as the patterns 4 * row0, ... of the list -> stats int64[3]"""
+        allow = np.ascontiguousarray(allow, dtype=np.uint32).reshape(-1, 4)
+        lens = np.ascontiguousarray(lens, dtype=np.int32)
+        strict = np.ascontiguousarray(strict, dtype=np.uint32)
+        rec_off = np.ascontiguousarray(rec_off, dtype=np.int64)
+        rec_len = np.ascontiguousarray(rec_len, dtype=np.int64)
+        amp = perf = None
+        words = 0
+        if mat is not None:
+            if len(rec_off) != mat.n_rec or not 0 <= row0 <= row0 + len(lens) // 4 <= mat.n_rows:
+                raise MpbError(-1, "pairs %d.. / %d records do not fit the %d x %d matrix" % (
+                    row0, len(rec_off), mat.n_rows, mat.n_rec))
+            off = row0 * mat.words * 4
+            amp, perf, words = C.c_void_p(mat.amp + off), C.c_void_p(mat.perf + off), mat.words
+        stats = np.zeros(3, np.int64)
+        check(load().mpb_pattern_cover_keep(self.h, len(lens), ptr(allow), ptr(lens), ptr(strict), v, stride,
+                                            len(rec_off), ptr(rec_off), ptr(rec_len), lo, hi, words, amp, perf,
+                                            int(max_sites), ptr(stats), sites.h, 4 * int(row0)))
         return stats
 
     def seqkeys(self, k: int, win_pos) -> np.ndarray:

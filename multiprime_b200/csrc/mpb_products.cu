@@ -624,19 +624,29 @@ __global__ void k_cover_join(const unsigned long long* __restrict__ key, long lo
     }
 }
 
-extern "C" int mpb_pattern_cover(mpb_msa* m, int32_t n_pat, const uint32_t* allow, const int32_t* lens,
-                                 const uint32_t* strict, int32_t v, int64_t stride, int32_t n_rec, const int64_t* rec_off,
-                                 const int64_t* rec_len, int32_t lo, int32_t hi, int64_t words, uint32_t* amp,
-                                 uint32_t* perf, int64_t max_sites, int64_t* stats) {
-    if (!m || !allow || !lens || !strict || !amp || !perf || !stats || (n_rec > 0 && (!rec_off || !rec_len)))
+// the site list of mpb_pattern_cover_keep (defined below)
+static int sites_check_block(const mpb_site_list* s, int32_t pat0, int32_t n_pat, const int32_t* lens, int32_t n_rec,
+                             const int64_t* rec_off, const int64_t* rec_len);
+static int sites_append(mpb_site_list* s, const unsigned long long* key, long long n, int pos_bits, int32_t pat0);
+
+// mpb_pattern_cover, and with a site list (list != NULL) mpb_pattern_cover_keep: the same search, filter, sort and join,
+// with the filtered sites also appended to the list; amp / perf NULL (keep only) stops after the append
+static int pattern_cover(mpb_msa* m, int32_t n_pat, const uint32_t* allow, const int32_t* lens, const uint32_t* strict,
+                         int32_t v, int64_t stride, int32_t n_rec, const int64_t* rec_off, const int64_t* rec_len,
+                         int32_t lo, int32_t hi, int64_t words, uint32_t* amp, uint32_t* perf, int64_t max_sites,
+                         int64_t* stats, mpb_site_list* list, int32_t pat0) {
+    const bool join = amp || perf || !list;
+    if (!m || !allow || !lens || !strict || (join && (!amp || !perf)) || !stats || (n_rec > 0 && (!rec_off || !rec_len)))
         return fail(MPB_EINVAL, "NULL argument");
     if (v < 0) return fail(MPB_EINVAL, "negative mismatch bound %d", v);
     if (n_pat < 4 || n_pat % 4) return fail(MPB_EINVAL, "%d patterns: four per pair are needed", n_pat);
     if (n_rec < 0 || (long long)n_rec > COVER_MAX_REC) return fail(MPB_EINVAL, "bad n_rec %d", n_rec);
-    if (words < (n_rec + 31) / 32) return fail(MPB_EINVAL, "%lld words hold fewer than %d records", (long long)words, n_rec);
+    if (join && words < (n_rec + 31) / 32)
+        return fail(MPB_EINVAL, "%lld words hold fewer than %d records", (long long)words, n_rec);
     if (lo < 1 || lo > hi) return fail(MPB_EINVAL, "product lengths %d..%d: need 0 < lo <= hi", lo, hi);
     if (max_sites < 0 || max_sites > (1ll << 31)) return fail(MPB_EINVAL, "max_sites %lld outside 0..2^31", (long long)max_sites);
-    if (!mpb_is_device_ptr(amp) || !mpb_is_device_ptr(perf)) return fail(MPB_EINVAL, "amp and perf must be device memory");
+    if (join && (!mpb_is_device_ptr(amp) || !mpb_is_device_ptr(perf)))
+        return fail(MPB_EINVAL, "amp and perf must be device memory");
     if (stride < 1 || stride > (1ll << 60) / (m->n_seq > 0 ? m->n_seq : 1))
         return fail(MPB_EINVAL, "%lld rows of stride %lld: the site key needs more than 64 bits", (long long)m->n_seq,
                     (long long)stride);
@@ -651,6 +661,8 @@ extern "C" int mpb_pattern_cover(mpb_msa* m, int32_t n_pat, const uint32_t* allo
     if (n_rec > 0 && rec_off[n_rec - 1] + rec_len[n_rec - 1] > m->n_seq * stride)  // keys and windows stay in pos_bits
         return fail(MPB_EINVAL, "record %d ends at %lld, past the %lld stream columns of the rows", n_rec - 1,
                     (long long)(rec_off[n_rec - 1] + rec_len[n_rec - 1]), (long long)(m->n_seq * stride));
+    if (list)
+        if (int rc = sites_check_block(list, pat0, n_pat, lens, n_rec, rec_off, rec_len)) return rc;
     mpb_ctx* ctx = m->ctx;
     CK(cudaSetDevice(ctx->device));
     for (int s = 0; s < 3; ++s) stats[s] = 0;
@@ -696,7 +708,9 @@ extern "C" int mpb_pattern_cover(mpb_msa* m, int32_t n_pat, const uint32_t* allo
     const long long n_key = (long long)nk[0];
     stats[1] = (int64_t)nk[1];
     stats[2] = n_key - (int64_t)nk[1];
-    if (stats[1] == 0 || stats[2] == 0) return 0;
+    if (list)
+        if (int rc = sites_append(list, k1.as<unsigned long long>(), n_key, pos_bits, pat0)) return rc;
+    if (!join || stats[1] == 0 || stats[2] == 0) return 0;
     {
         unsigned long long *a = k1.as<unsigned long long>(), *b = k2.as<unsigned long long>();
         const int rc = cub_run(ctx, "k_cover_sort", tmp, [&](void* t, size_t& bytes) {
@@ -710,6 +724,25 @@ extern "C" int mpb_pattern_cover(mpb_msa* m, int32_t n_pat, const uint32_t* allo
                      (long long)words, amp, perf);
     CK(cudaStreamSynchronize(ctx->stream));
     return 0;
+}
+
+extern "C" int mpb_pattern_cover(mpb_msa* m, int32_t n_pat, const uint32_t* allow, const int32_t* lens,
+                                 const uint32_t* strict, int32_t v, int64_t stride, int32_t n_rec, const int64_t* rec_off,
+                                 const int64_t* rec_len, int32_t lo, int32_t hi, int64_t words, uint32_t* amp,
+                                 uint32_t* perf, int64_t max_sites, int64_t* stats) {
+    return pattern_cover(m, n_pat, allow, lens, strict, v, stride, n_rec, rec_off, rec_len, lo, hi, words, amp, perf,
+                         max_sites, stats, nullptr, 0);
+}
+
+extern "C" int mpb_pattern_cover_keep(mpb_msa* m, int32_t n_pat, const uint32_t* allow, const int32_t* lens,
+                                      const uint32_t* strict, int32_t v, int64_t stride, int32_t n_rec,
+                                      const int64_t* rec_off, const int64_t* rec_len, int32_t lo, int32_t hi, int64_t words,
+                                      uint32_t* amp, uint32_t* perf, int64_t max_sites, int64_t* stats,
+                                      mpb_site_list* list, int32_t pat0) {
+    if (!list) return fail(MPB_EINVAL, "NULL site list");
+    if ((amp == nullptr) != (perf == nullptr)) return fail(MPB_EINVAL, "amp and perf: both or neither");
+    return pattern_cover(m, n_pat, allow, lens, strict, v, stride, n_rec, rec_off, rec_len, lo, hi, words, amp, perf,
+                         max_sites, stats, list, pat0);
 }
 
 // gains[2i] = popcount(amp[cand[i]] & ~covered), gains[2i+1] = popcount(perf[cand[i]] & ~covered_perfect): one warp per
@@ -791,6 +824,353 @@ extern "C" int mpb_cover_take(mpb_ctx* ctx, const uint32_t* amp, const uint32_t*
     CK(cudaSetDevice(ctx->device));
     MPB_LAUNCH(ctx, k_cover_take, grid_of(words), 256, 0, amp + row * words, perf + row * words, (long long)words, covered,
                covered_perfect);
+    CK(cudaStreamSynchronize(ctx->stream));
+    return 0;
+}
+
+
+// ---- mpb_site_list: the kept sites of mpb_pattern_cover_keep and their joins (primer_select.py --cross / --background)
+// The list holds the filtered sites of every pattern of a panel over one set of records, in one 64-bit key each:
+//     stream position << (pat_bits + 4) | pattern << 4 | mismatches
+//   keep   mpb_pattern_cover_keep appends the keys of its block (k_sites_keep re-packs the cover keys, pattern + pat0);
+//   seal   one cub::DeviceRadixSort of all the keys puts them in stream order, and k_sites_count counts each pattern's
+//          sites (the capacity of a pair's pick);
+//   cross  k_sites_pick gathers the sites of the taken pair's four patterns, then k_sites_cross gives every one of them
+//          a warp that walks the stream-ordered list from its site over its product window: forward from a left site
+//          to the right sites that can close a product with it, backward from a right site to the left sites.  The
+//          window is a contiguous run of the list, so the lanes read consecutive keys; a key of an eligible pair
+//          (bitmask in shared memory) that closes a product sets one of its pair's 8 bits (check, then atomicOr);
+//   own    k_sites_repack re-keys the list pattern-first, one sort puts each pattern's sites in stream order, and
+//          k_sites_own binary-searches, for every left site, the runs of its own pair's two right patterns, as
+//          k_cover_join does for one of them.
+// A pattern's primer: 4q (F, left), 4q+1 (R, right), 4q+2 (R, left), 4q+3 (F, right); 0 = F, 1 = R.
+struct mpb_site_list {
+    mpb_ctx* ctx;
+    int32_t n_pat, n_rec;
+    int64_t n_pos;
+    int pat_bits, pos_bits;
+    std::vector<int32_t> h_lens;
+    std::vector<int64_t> h_off, h_len, count;  // count: sites per pattern, after the seal
+    DMem keys, d_lens, d_off, d_len;
+    long long n = 0;
+    bool sealed = false;
+};
+
+__device__ __forceinline__ int primer_of(int p) { return ((p & 3) == 1 || (p & 3) == 2) ? 1 : 0; }
+
+// bit b of pair c's byte in out[] (4 pairs per word), read first so a bit that is set costs no atomic
+__device__ __forceinline__ void set_pair_bit(uint32_t* out, int c, int b) {
+    const uint32_t bit = 1u << ((c & 3) * 8 + b);
+    if (!(__ldcg(out + (c >> 2)) & bit)) atomicOr(out + (c >> 2), bit);
+}
+
+__global__ void k_sites_keep(const unsigned long long* __restrict__ in, long long n, int in_pos_bits, int pat_bits,
+                             int pat0, unsigned long long* __restrict__ out) {
+    const unsigned long long pos_mask = (1ull << in_pos_bits) - 1;
+    for (long long k = (long long)blockIdx.x * blockDim.x + threadIdx.x; k < n; k += (long long)gridDim.x * blockDim.x) {
+        const unsigned long long kk = in[k];
+        const unsigned long long p = (kk >> (in_pos_bits + 4)) + (unsigned long long)pat0, g = (kk >> 4) & pos_mask;
+        out[k] = g << (pat_bits + 4) | p << 4 | (kk & 15);
+    }
+}
+
+__global__ void k_sites_count(const unsigned long long* __restrict__ key, long long n, int pat_bits,
+                              unsigned long long* __restrict__ count) {
+    const unsigned long long pat_mask = (1ull << pat_bits) - 1;
+    for (long long k = (long long)blockIdx.x * blockDim.x + threadIdx.x; k < n; k += (long long)gridDim.x * blockDim.x)
+        atomicAdd(count + ((key[k] >> 4) & pat_mask), 1ull);
+}
+
+__global__ void k_sites_pick(const unsigned long long* __restrict__ key, long long n, int pat_bits, int p0,
+                             long long* __restrict__ pick, unsigned long long* __restrict__ n_pick) {
+    const unsigned long long pat_mask = (1ull << pat_bits) - 1;
+    for (long long k = (long long)blockIdx.x * blockDim.x + threadIdx.x; k < n; k += (long long)gridDim.x * blockDim.x) {
+        const int p = (int)((__ldg(key + k) >> 4) & pat_mask);
+        if (p >= p0 && p < p0 + 4) pick[atomicAdd(n_pick, 1ull)] = k;
+    }
+}
+
+#define CROSS_WARPS 8
+__global__ void __launch_bounds__(CROSS_WARPS * 32)
+k_sites_cross(const unsigned long long* __restrict__ key, long long n, const long long* __restrict__ pick, long long n_pick,
+              int pat_bits, const int32_t* __restrict__ pat_len, const int64_t* __restrict__ off,
+              const int64_t* __restrict__ len, int n_rec, int lo, int hi, const uint32_t* __restrict__ elig, int elig_words,
+              uint32_t* __restrict__ out) {
+    extern __shared__ uint32_t s_elig[];
+    for (int w = threadIdx.x; w < elig_words; w += blockDim.x) s_elig[w] = __ldg(elig + w);
+    __syncthreads();
+    const long long i = (long long)blockIdx.x * CROSS_WARPS + (threadIdx.x >> 5);
+    if (i >= n_pick) return;  // the whole warp
+    const int lane = threadIdx.x & 31, sh = pat_bits + 4;
+    const unsigned long long pat_mask = (1ull << pat_bits) - 1;
+    const long long k = __ldg(pick + i);
+    const unsigned long long kk = __ldg(key + k);
+    const long long g = (long long)(kk >> sh);
+    const int p = (int)((kk >> 4) & pat_mask), lt = __ldg(pat_len + p), pt = primer_of(p);
+    const int r = find_record(off, n_rec, g);
+    const long long start = __ldg(off + r), end = start + __ldg(len + r);
+    if ((p & 1) == 0) {
+        // a left site of the taken pair at g: right sites y >= g + lt with y + L - g in [lo, hi], y + L <= end
+        const long long last = min(g + (long long)hi, end) - 1;
+        for (long long b = k + 1 + lane;; b += 32) {
+            bool past = b >= n;
+            if (!past) {
+                const unsigned long long rk = __ldg(key + b);
+                const long long y = (long long)(rk >> sh);
+                past = y > last;
+                const int q = (int)((rk >> 4) & pat_mask), c = q >> 2;
+                if (!past && (q & 1) && (s_elig[c >> 5] >> (c & 31) & 1)) {
+                    const long long l = y + __ldg(pat_len + q) - g;
+                    if (y >= g + lt && l >= lo && l <= hi && g + l <= end) set_pair_bit(out, c, primer_of(q) << 1 | pt);
+                }
+            }
+            if (__any_sync(0xFFFFFFFFu, past)) break;  // the list is in stream order: every later key is past too
+        }
+    } else {
+        // a right site of the taken pair at g: left sites x >= start with x + L <= g and g + lt - x in [lo, hi]
+        const long long first = max(start, g + lt - (long long)hi);
+        for (long long b = k - 1 - lane;; b -= 32) {
+            bool past = b < 0;
+            if (!past) {
+                const unsigned long long lk = __ldg(key + b);
+                const long long x = (long long)(lk >> sh);
+                past = x < first;
+                const int q = (int)((lk >> 4) & pat_mask), c = q >> 2;
+                if (!past && !(q & 1) && (s_elig[c >> 5] >> (c & 31) & 1)) {
+                    const long long l = g + lt - x;
+                    if (x + __ldg(pat_len + q) <= g && l >= lo && l <= hi)
+                        set_pair_bit(out, c, 4 | primer_of(q) << 1 | pt);
+                }
+            }
+            if (__any_sync(0xFFFFFFFFu, past)) break;
+        }
+    }
+}
+
+__global__ void k_sites_repack(const unsigned long long* __restrict__ in, long long n, int pat_bits, int pos_bits,
+                               unsigned long long* __restrict__ out) {
+    const unsigned long long pat_mask = (1ull << pat_bits) - 1;
+    for (long long k = (long long)blockIdx.x * blockDim.x + threadIdx.x; k < n; k += (long long)gridDim.x * blockDim.x) {
+        const unsigned long long kk = in[k];
+        out[k] = ((kk >> 4) & pat_mask) << (pos_bits + 4) | (kk >> (pat_bits + 4)) << 4 | (kk & 15);
+    }
+}
+
+__global__ void k_sites_own(const unsigned long long* __restrict__ key, long long n, int pos_bits,
+                            const int32_t* __restrict__ pat_len, const int64_t* __restrict__ off,
+                            const int64_t* __restrict__ len, int n_rec, int lo, int hi, uint32_t* __restrict__ out) {
+    const unsigned long long pos_mask = (1ull << pos_bits) - 1;
+    for (long long k = (long long)blockIdx.x * blockDim.x + threadIdx.x; k < n; k += (long long)gridDim.x * blockDim.x) {
+        const unsigned long long kk = key[k];
+        const int p = (int)(kk >> (pos_bits + 4));
+        if (p & 1) continue;
+        const long long g = (long long)((kk >> 4) & pos_mask);
+        const int r = find_record(off, n_rec, g);
+        const long long end = __ldg(off + r) + __ldg(len + r);
+        const int ll = __ldg(pat_len + p), c = p >> 2;
+        for (int rp = (p & ~3) + 1; rp < (p & ~3) + 4; rp += 2) {  // RC(R) and RC(F) of the site's own pair
+            const int b = primer_of(p) << 1 | primer_of(rp);
+            if (__ldcg(out + (c >> 2)) >> ((c & 3) * 8 + b) & 1) continue;
+            const int rl = __ldg(pat_len + rp);
+            const long long ylo = g + max(ll, lo - rl), yhi = min(g + (long long)hi - rl, end - rl);
+            if (ylo > yhi) continue;
+            const unsigned long long base = (unsigned long long)rp << (pos_bits + 4);
+            const unsigned long long want = base | (unsigned long long)ylo << 4, last = base | (unsigned long long)yhi << 4 | 15;
+            long long q0 = 0, q1 = n;
+            while (q0 < q1) {
+                const long long mid = (q0 + q1) >> 1;
+                if (__ldg(key + mid) < want) q0 = mid + 1;
+                else q1 = mid;
+            }
+            if (q0 < n && __ldg(key + q0) <= last) set_pair_bit(out, c, b);
+        }
+    }
+}
+
+static int sites_no_memory(const char* what, long long sites, long long bytes) {
+    cudaGetLastError();
+    return fail(MPB_ENOMEM, "the site list's %s of %lld sites needs %lld bytes of device memory", what, sites, bytes);
+}
+
+static int sites_check_block(const mpb_site_list* s, int32_t pat0, int32_t n_pat, const int32_t* lens, int32_t n_rec,
+                             const int64_t* rec_off, const int64_t* rec_len) {
+    if (s->sealed) return fail(MPB_EINVAL, "the site list is sealed: no site can be added");
+    if (pat0 < 0 || pat0 % 4 || (long long)pat0 + n_pat > s->n_pat)
+        return fail(MPB_EINVAL, "patterns %d..%lld outside the site list's 0..%d", pat0, (long long)pat0 + n_pat - 1,
+                    s->n_pat - 1);
+    for (int32_t p = 0; p < n_pat; ++p)
+        if (lens[p] != s->h_lens[pat0 + p])
+            return fail(MPB_EINVAL, "pattern %d: length %d, the site list has %d", pat0 + p, lens[p], s->h_lens[pat0 + p]);
+    if (n_rec != s->n_rec) return fail(MPB_EINVAL, "%d records, the site list has %d", n_rec, s->n_rec);
+    for (int32_t r = 0; r < n_rec; ++r)
+        if (rec_off[r] != s->h_off[r] || rec_len[r] != s->h_len[r])
+            return fail(MPB_EINVAL, "record %d differs from the site list's", r);
+    return 0;
+}
+
+static int sites_append(mpb_site_list* s, const unsigned long long* key, long long n, int pos_bits, int32_t pat0) {
+    if (n == 0) return 0;
+    mpb_ctx* ctx = s->ctx;
+    const long long need = s->n + n;
+    if ((size_t)need * 8 > s->keys.bytes) {
+        const long long want = need + need / 2;  // room for the next blocks: geometric growth
+        if (s->keys.grow((size_t)want * 8, (size_t)s->n * 8, ctx->stream) != cudaSuccess &&
+            s->keys.grow((size_t)need * 8, (size_t)s->n * 8, ctx->stream) != cudaSuccess)
+            return sites_no_memory("keys", need, need * 8);
+    }
+    MPB_LAUNCH(ctx, k_sites_keep, grid_of(n), 256, 0, key, n, pos_bits, s->pat_bits, (int)pat0,
+               s->keys.as<unsigned long long>() + s->n);
+    s->n = need;
+    return 0;
+}
+
+extern "C" int mpb_site_list_create(mpb_ctx* ctx, int32_t n_pat, const int32_t* lens, int64_t n_pos, int32_t n_rec,
+                                    const int64_t* rec_off, const int64_t* rec_len, mpb_site_list** out) {
+    if (!ctx || !lens || !out || (n_rec > 0 && (!rec_off || !rec_len))) return fail(MPB_EINVAL, "NULL argument");
+    *out = nullptr;
+    if (n_pat < 4 || n_pat % 4) return fail(MPB_EINVAL, "%d patterns: four per pair are needed", n_pat);
+    if (n_rec < 0 || (long long)n_rec > COVER_MAX_REC) return fail(MPB_EINVAL, "bad n_rec %d", n_rec);
+    if (n_pos < 1) return fail(MPB_EINVAL, "bad n_pos %lld", (long long)n_pos);
+    const int pat_bits = bits_for(n_pat), pos_bits = bits_for(n_pos);
+    if (pat_bits + pos_bits + 4 > 64)
+        return fail(MPB_EINVAL, "%d patterns over %lld stream columns: the site key needs %d + %d + 4 > 64 bits", n_pat,
+                    (long long)n_pos, pat_bits, pos_bits);
+    for (int32_t p = 0; p < n_pat; ++p)
+        if (lens[p] < 1 || lens[p] > 32) return fail(MPB_EINVAL, "pattern %d: length %d outside 1..32", p, lens[p]);
+    for (int32_t r = 0; r < n_rec; ++r)
+        if (rec_len[r] < 0 || rec_off[r] < 0 || (r > 0 && rec_off[r] < rec_off[r - 1] + rec_len[r - 1]))
+            return fail(MPB_EINVAL, "record %d: offset %lld / length %lld overlap the record before it", r,
+                        (long long)rec_off[r], (long long)rec_len[r]);
+    if (n_rec > 0 && rec_off[n_rec - 1] + rec_len[n_rec - 1] > n_pos)
+        return fail(MPB_EINVAL, "record %d ends past the %lld stream columns", n_rec - 1, (long long)n_pos);
+    CK(cudaSetDevice(ctx->device));
+    mpb_site_list* s = new mpb_site_list();
+    s->ctx = ctx, s->n_pat = n_pat, s->n_rec = n_rec, s->n_pos = n_pos, s->pat_bits = pat_bits, s->pos_bits = pos_bits;
+    s->h_lens.assign(lens, lens + n_pat);
+    s->h_off.assign(rec_off, rec_off + n_rec);
+    s->h_len.assign(rec_len, rec_len + n_rec);
+    cudaError_t e = s->d_lens.reserve(n_pat * 4);
+    if (e == cudaSuccess) e = s->d_off.reserve(n_rec * 8 + 8);
+    if (e == cudaSuccess) e = s->d_len.reserve(n_rec * 8 + 8);
+    if (e == cudaSuccess) e = cudaMemcpy(s->d_lens.p, lens, n_pat * 4, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess && n_rec) e = cudaMemcpy(s->d_off.p, rec_off, n_rec * 8, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess && n_rec) e = cudaMemcpy(s->d_len.p, rec_len, n_rec * 8, cudaMemcpyHostToDevice);
+    if (e != cudaSuccess) {
+        delete s;
+        CK(e);
+    }
+    *out = s;
+    return 0;
+}
+
+extern "C" void mpb_site_list_destroy(mpb_site_list* s) {
+    if (!s) return;
+    cudaSetDevice(s->ctx->device);
+    delete s;
+}
+
+extern "C" int mpb_site_list_seal(mpb_site_list* s, int64_t* n_sites) {
+    if (!s || !n_sites) return fail(MPB_EINVAL, "NULL argument");
+    if (s->sealed) return fail(MPB_EINVAL, "the site list is sealed already");
+    mpb_ctx* ctx = s->ctx;
+    CK(cudaSetDevice(ctx->device));
+    s->count.assign(s->n_pat, 0);
+    if (s->n > 0) {
+        DMem alt, tmp, cnt;
+        if (alt.reserve((size_t)s->n * 8) != cudaSuccess) return sites_no_memory("sort buffer", s->n, s->n * 8);
+        unsigned long long *a = s->keys.as<unsigned long long>(), *b = alt.as<unsigned long long>();
+        const long long n = s->n;
+        const int bits = s->pat_bits + s->pos_bits + 4;
+        if (int rc = cub_run(ctx, "k_sites_seal", tmp, [&](void* t, size_t& bytes) {
+                return cub::DeviceRadixSort::SortKeys(t, bytes, a, b, n, 0, bits, ctx->stream);
+            }))
+            return rc;
+        std::swap(s->keys.p, alt.p);
+        std::swap(s->keys.bytes, alt.bytes);
+        CK(cnt.reserve((size_t)s->n_pat * 8));
+        CK(cudaMemsetAsync(cnt.p, 0, (size_t)s->n_pat * 8, ctx->stream));
+        MPB_LAUNCH(ctx, k_sites_count, grid_of(n), 256, 0, s->keys.as<unsigned long long>(), n, s->pat_bits,
+                   cnt.as<unsigned long long>());
+        CK(cudaMemcpyAsync(s->count.data(), cnt.p, (size_t)s->n_pat * 8, cudaMemcpyDeviceToHost, ctx->stream));
+        CK(cudaStreamSynchronize(ctx->stream));
+    }
+    s->sealed = true;
+    *n_sites = s->n;
+    return 0;
+}
+
+extern "C" int mpb_site_list_keys(mpb_site_list* s, int64_t cap, uint64_t* keys, int64_t* n_sites) {
+    if (!s || !n_sites || (cap > 0 && !keys)) return fail(MPB_EINVAL, "NULL argument");
+    *n_sites = s->n;
+    const long long k = cap < s->n ? cap : s->n;
+    if (k <= 0) return 0;
+    CK(cudaSetDevice(s->ctx->device));
+    CK(cudaMemcpyAsync(keys, s->keys.p, (size_t)k * 8, cudaMemcpyDeviceToHost, s->ctx->stream));
+    CK(cudaStreamSynchronize(s->ctx->stream));
+    return 0;
+}
+
+static int sites_join_args(const mpb_site_list* s, int32_t lo, int32_t hi) {
+    if (!s->sealed) return fail(MPB_EINVAL, "the site list is not sealed");
+    if (lo < 1 || lo > hi) return fail(MPB_EINVAL, "product lengths %d..%d: need 0 < lo <= hi", lo, hi);
+    return 0;
+}
+
+extern "C" int mpb_sites_cross(mpb_site_list* s, int32_t lo, int32_t hi, int32_t pair, const uint32_t* eligible,
+                               uint8_t* bits) {
+    if (!s || !eligible || !bits) return fail(MPB_EINVAL, "NULL argument");
+    if (int rc = sites_join_args(s, lo, hi)) return rc;
+    const int n_pairs = s->n_pat / 4, words = (n_pairs + 31) / 32;
+    if (pair < 0 || pair >= n_pairs) return fail(MPB_EINVAL, "pair %d outside 0..%d", pair, n_pairs - 1);
+    memset(bits, 0, n_pairs);
+    long long n_pick = 0;
+    for (int p = 4 * pair; p < 4 * pair + 4; ++p) n_pick += s->count[p];
+    if (n_pick == 0) return 0;
+    mpb_ctx* ctx = s->ctx;
+    CK(cudaSetDevice(ctx->device));
+    DMem d_pick, d_n, d_elig, d_out;
+    if (d_pick.reserve((size_t)n_pick * 8) != cudaSuccess) return sites_no_memory("pick", n_pick, n_pick * 8);
+    CK(d_n.reserve(8));
+    CK(d_elig.reserve((size_t)words * 4));
+    CK(d_out.reserve((size_t)(n_pairs + 3) / 4 * 4));
+    CK(cudaMemsetAsync(d_n.p, 0, 8, ctx->stream));
+    CK(cudaMemsetAsync(d_out.p, 0, (size_t)(n_pairs + 3) / 4 * 4, ctx->stream));
+    CK(cudaMemcpyAsync(d_elig.p, eligible, (size_t)words * 4, cudaMemcpyHostToDevice, ctx->stream));
+    MPB_LAUNCH(ctx, k_sites_pick, grid_of(s->n), 256, 0, s->keys.as<unsigned long long>(), (long long)s->n, s->pat_bits,
+               4 * pair, d_pick.as<long long>(), d_n.as<unsigned long long>());
+    MPB_LAUNCH(ctx, k_sites_cross, (unsigned)((n_pick + CROSS_WARPS - 1) / CROSS_WARPS), CROSS_WARPS * 32,
+               (size_t)words * 4, s->keys.as<unsigned long long>(), (long long)s->n, d_pick.as<long long>(), n_pick,
+               s->pat_bits, s->d_lens.as<int32_t>(), s->d_off.as<int64_t>(), s->d_len.as<int64_t>(), (int)s->n_rec,
+               (int)lo, (int)hi, d_elig.as<uint32_t>(), words, d_out.as<uint32_t>());
+    CK(cudaMemcpyAsync(bits, d_out.p, n_pairs, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    return 0;
+}
+
+extern "C" int mpb_sites_own(mpb_site_list* s, int32_t lo, int32_t hi, uint8_t* bits) {
+    if (!s || !bits) return fail(MPB_EINVAL, "NULL argument");
+    if (int rc = sites_join_args(s, lo, hi)) return rc;
+    const int n_pairs = s->n_pat / 4;
+    memset(bits, 0, n_pairs);
+    if (s->n == 0) return 0;
+    mpb_ctx* ctx = s->ctx;
+    CK(cudaSetDevice(ctx->device));
+    const long long n = s->n;
+    DMem k1, k2, tmp, d_out;
+    if (k1.reserve((size_t)n * 8) != cudaSuccess || k2.reserve((size_t)n * 8) != cudaSuccess)
+        return sites_no_memory("pattern-first copy", n, 2 * n * 8);
+    CK(d_out.reserve((size_t)(n_pairs + 3) / 4 * 4));
+    CK(cudaMemsetAsync(d_out.p, 0, (size_t)(n_pairs + 3) / 4 * 4, ctx->stream));
+    unsigned long long *a = k1.as<unsigned long long>(), *b = k2.as<unsigned long long>();
+    MPB_LAUNCH(ctx, k_sites_repack, grid_of(n), 256, 0, s->keys.as<unsigned long long>(), n, s->pat_bits, s->pos_bits, a);
+    const int key_bits = s->pat_bits + s->pos_bits + 4;
+    if (int rc = cub_run(ctx, "k_sites_own_sort", tmp, [&](void* t, size_t& bytes) {
+            return cub::DeviceRadixSort::SortKeys(t, bytes, a, b, n, 0, key_bits, ctx->stream);
+        }))
+        return rc;
+    MPB_LAUNCH(ctx, k_sites_own, grid_of(n), 256, 0, b, n, s->pos_bits, s->d_lens.as<int32_t>(), s->d_off.as<int64_t>(),
+               s->d_len.as<int64_t>(), (int)s->n_rec, (int)lo, (int)hi, d_out.as<uint32_t>());
+    CK(cudaMemcpyAsync(bits, d_out.p, n_pairs, cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
     return 0;
 }

@@ -188,3 +188,24 @@ def pcr_candidate_pool(n_pairs: int = 2048, length: int = 10_000, seed: int = 20
         r = "".join("ACGT"[3 - x] for x in src[b:b + 20][::-1])
         pairs["cand%04d_v%d" % (q, q % 9)] = (f, r)
     return pairs
+
+
+def write_pcr_background(path: str, n_random: int = 256, random_length: int = 10_000, n_copies: int = 4,
+                         copy_span=(0, 3000), divergence: float = 0.02, length: int = 10_000, seed: int = 20241015):
+    """A background for primer_select --background (tools/bench_select_specific.py): n_random records of uniform random
+    bases, which no 20-mer of the pool binds with a few mismatches by chance, and n_copies copies of root[copy_span]
+    of write_pcr_targets (the generator's first draw, replayed) with `divergence` point substitutions each, so the
+    candidates of pcr_candidate_pool whose sites both fall in copy_span have products there (off-target) and the
+    others do not.  Returns the number of records."""
+    rng = np.random.Generator(np.random.PCG64([seed, 0x9C2]))
+    root = rng.integers(0, 4, length).astype(np.uint8)
+    bg = np.random.Generator(np.random.PCG64([seed, 0xB6]))
+    with open(path, "w") as fh:
+        for k in range(n_random):
+            fh.write(">random%05d\n%s\n" % (k, "".join("ACGT"[x] for x in bg.integers(0, 4, random_length))))
+        for k in range(n_copies):
+            x = root[copy_span[0]:copy_span[1]].copy()
+            hit = bg.random(len(x)) < divergence
+            x[hit] = (x[hit] + bg.integers(1, 4, int(hit.sum()))) % 4
+            fh.write(">root_copy%d\n%s\n" % (k, "".join("ACGT"[c] for c in x)))
+    return n_random + n_copies
